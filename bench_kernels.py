@@ -3,6 +3,8 @@
 times every hot-path kernel alone on the 256^3 cavity with CUDA events and reports achieved
 ALGORITHMIC GB/s (SURVEY.md section 8d byte counts) against the measured HBM peak.
   python bench_kernels.py [--n 256] [--reps 20] > gpurun_out/kernels.json
+The two sweeps of the fused PCG iteration are timed inside a 50-iteration solve with torch.profiler, in a process of
+its own (`--pcg-sweeps` runs only that part): per-sweep time, layout bytes and GB/s, and the gaps between the sweeps.
 Run it under `ncu --metrics gpu__time_duration.sum` for the matching launch list."""
 import argparse
 import importlib
@@ -16,11 +18,100 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
 
+def pcg_sweep_bytes(info):
+    """Bytes the banded layout moves in the two sweeps of one fused PCG iteration (single domain: every entry is
+    local).  Stream: 8 B coefficient + 2 B column per entry.  Halo: a 4 B haloIdx per column plus the vectors the
+    op's stage() reads there.  Own rows: the vectors read and written while staging and in finish()."""
+    nPad, nE, nH = info["nPadRows"], info["nEntries"], info["nHalo"]
+    # A (PcgAinvOp): own rows read rOld, w, p, psi, rD and write psi, rNew, z; halo reads w, rOld, rD
+    a = 64 * nPad + 10 * nE + (4 + 24) * nH
+    # B (PcgAmulOp): own rows read z, pOld, diag and write pNew, w; halo reads z, pOld
+    b = 40 * nPad + 10 * nE + (4 + 16) * nH
+    return a, b
+
+
+def pcg_sweeps(n, iters):
+    """Per-kernel times of the two fused PCG sweeps inside an n^3, `iters`-iteration PCG+DIC solve, from
+    torch.profiler (CUDA activities), and the gaps between consecutive sweeps.  Prints one JSON object."""
+    import tempfile
+
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    capi = importlib.import_module("rapidcfd-dev_b200.capi")
+    meshmod = importlib.import_module("rapidcfd-dev_b200.mesh")
+    mesh = meshmod.hex_mesh(n)
+    ctx = capi.Context(0)
+    dev = ctx.device
+    tt = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
+    addr = capi.mesh_to_device(ctx, mesh)
+    cp = meshmod.pressure_laplacian(mesh)
+    mat = capi.LduMatrix(addr)
+    mat.set(tt(cp["diag"]), tt(cp["upper"]))
+    b = tt(meshmod.cell_field_global(mesh, 9))
+    psi = torch.zeros(mesh.nCells, dtype=torch.float64, device=dev)
+    kw = dict(tolerance=0.0, maxIter=iters - 1)
+    for _ in range(2):
+        psi.zero_()
+        mat.solve("PCG", "DIC", psi, b, **kw)
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(3):
+            psi.zero_()
+            mat.solve("PCG", "DIC", psi, b, **kw)
+        torch.cuda.synchronize()
+    with tempfile.TemporaryDirectory() as td:
+        path = os.path.join(td, "trace.json")
+        prof.export_chrome_trace(path)
+        with open(path) as f:
+            trace = json.load(f)
+    kern = sorted((e for e in trace.get("traceEvents", []) if e.get("cat") == "kernel"), key=lambda e: e["ts"])
+    which = lambda e: "A" if "PcgAinvOp" in e["name"] else ("B" if "PcgAmulOp" in e["name"] else None)
+    dur = {"A": [], "B": []}
+    gap = {"A->B": [], "B->A": []}
+    prev = None
+    for e in kern:
+        w = which(e)
+        if w is None:
+            prev = None
+            continue
+        dur[w].append(e["dur"])
+        if prev is not None and which(prev) != w:
+            gap[f"{which(prev)}->{w}"].append(e["ts"] - (prev["ts"] + prev["dur"]))
+        prev = e
+    info = addr.info()
+    bytesA, bytesB = pcg_sweep_bytes(info)
+    med = lambda v: float(np.median(v)) if v else float("nan")
+    rows = []
+    for w, nm, nb in (("A", "PCG sweep A (AINV + r/psi update)", bytesA), ("B", "PCG sweep B (p update + Amul)", bytesB)):
+        us = med(dur[w])
+        rows.append({"kernel": nm, "layout_bytes": int(nb), "us_median": us, "us_min": min(dur[w], default=float("nan")),
+                     "launches": len(dur[w]), "GBps": nb / (us * 1e-6) / 1e9})
+    out = {"n": n, "iters": iters, "layout": info, "sweeps": rows,
+           "gap_us_median": {k: med(v) for k, v in gap.items()}, "gaps": {k: len(v) for k, v in gap.items()},
+           "iteration_us": med(dur["A"]) + med(dur["B"]) + med(gap["A->B"]) + med(gap["B->A"])}
+    mat.close()
+    addr.close()
+    ctx.close()
+    print(json.dumps(out), flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--n", type=int, default=256)
     ap.add_argument("--reps", type=int, default=20)
+    ap.add_argument("--pcg-sweeps", action="store_true",
+                    help="only the per-sweep attribution of the fused PCG iteration (torch.profiler)")
     args = ap.parse_args()
+    if args.pcg_sweeps:
+        return pcg_sweeps(args.n, 50)
+    import subprocess
+    # the profiler runs in a process of its own: tracing must not slow down the event-timed rows below
+    sw = subprocess.run([sys.executable, os.path.abspath(__file__), "--pcg-sweeps", "--n", str(args.n)],
+                        capture_output=True, text=True)
+    sweeps = json.loads(sw.stdout.strip().splitlines()[-1]) if sw.returncode == 0 else {"error": sw.stderr[-2000:]}
+    for r in sweeps.get("sweeps", []):
+        print(f"{r['kernel']:34s} {r['us_median']:9.1f} us  {r['GBps']:8.1f} GB/s (layout bytes)", file=sys.stderr)
+    print("gaps between sweeps (us):", sweeps.get("gap_us_median"), file=sys.stderr)
     import torch
     capi = importlib.import_module("rapidcfd-dev_b200.capi")
     meshmod = importlib.import_module("rapidcfd-dev_b200.mesh")
@@ -209,7 +300,8 @@ def main():
         fvm_error = repr(e)
         print("fvMatrix glue:", fvm_error, file=sys.stderr)
     solves["fvMatrix_glue_error"] = fvm_error
-    print(json.dumps({"n": n, "peak_gbs": peak, "peak_source": peak_src, "kernels": rows, "solves": solves}))
+    print(json.dumps({"n": n, "peak_gbs": peak, "peak_source": peak_src, "pcg_sweeps": sweeps, "kernels": rows,
+                      "solves": solves}))
     addr.close()
     ctx.close()
 

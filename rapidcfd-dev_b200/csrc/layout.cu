@@ -119,11 +119,14 @@ int pick_band_rows(int nCells, int smCount, int packCtas)
     // A sweep is one CTA per band, 6 resident per SM (792 slots on an H100 with 132 SMs).  Measured on one H100 80GB HBM3
     // (400 W power limit), bench.py --steps 20, Mcell-iters/s with matrix_set, one sample each:
     //   128^3:  512 rows (this rule) 9.9 k | 1024 rows 9.8 k | 2048 rows 9.2 k | 2688 rows (one wave, 781 CTAs) 9.0 k
-    //   256^3: 1024 rows 10.4 k | 2048 rows (this rule) 9.9 k | 2688 rows 9.3 k
+    //   256^3: 1024 rows 10.4 k | 2048 rows 9.9 k | 2688 rows 9.3 k
+    // and at a 700 W power limit, 256^3, alternating runs: 1024 rows (this rule) 11.66-11.68 k (3 runs) | 2048 rows 11.01 k (4 runs).
     // A mesh that fits one wave is best served by exactly one (every CTA resident at once, fewer partial sums for
     // the scalar step).  Beyond that, whole waves are the WORST choice -- the CTAs of a wave stage and stream in lock-step, so the
     // SM alternates between a latency-bound and a bandwidth-bound phase -- and 4+ waves of smaller bands, which drift out of
-    // phase, are best; the bands grow to 2048 rows as the mesh allows.
+    // phase, are best; the bands grow to 1024 rows as the mesh allows.  At 256^3 a 1024-row band's sweep A (the AINV
+    // sweep, whose staging phase carries most of its vector bytes) takes 782 us against 849 us for 2048 rows; sweep B
+    // 583 against 597 us (torch.profiler, bench_kernels.py --pcg-sweeps): 20 waves drift apart better than 10.
     // the packing CTAs of the fused halo send share the grid with the bands: keep bands + packers within the one wave
     const long long slots = (long long)(smCount > 0 ? smCount : 132) * 6 - packCtas;
     const long long maxRows = 2432; // the tile of a band + its halo must leave room for 6 CTAs per SM
@@ -134,7 +137,7 @@ int pick_band_rows(int nCells, int smCount, int packCtas)
     }
     const long long target = nCells / (slots * 4);
     int b = SLICE_ROWS;
-    while (b * 2 <= target && b < 2048) b *= 2;
+    while (b * 2 <= target && b < 1024) b *= 2;
     return b;
 }
 
