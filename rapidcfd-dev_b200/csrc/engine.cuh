@@ -95,30 +95,40 @@ __device__ __forceinline__ void block_reduce_store(double (&red)[NRED], double *
 
 // ---------------------------------------------------------------------------
 // Op concept
-//   static constexpr int  NVEC   1 or 2 vectors staged in shared memory
+//   static constexpr bool STAGED true: one vector is staged in shared memory (a = its value)
 //   static constexpr int  NRED   number of fused reductions (0..3)
 //   static constexpr bool LOCAL  true: owner/neighbour entries only (no interfaces)
 //   const int *stop              device flag; kernel exits at once when *stop != 0
+//   int waitHalo                 1: a peer-memory halo exchange of the staged vector is in flight
 //   bool prologue(L)             runs first in every CTA (default: nothing); false => the CTA exits
 //   double *partials             [nBands*NRED]
-//   void   stage(int g, double &a, double &b)        value(s) of extended index g
-//   void   stage_own(int r, double2 &a, double2 &b)  rows r, r+1 of the own band (may
-//                                                    also write a fused vector update)
-//   double init(int r, double a, double b)           start of the row sum
-//   double term(double acc, double v, double a, double b)   acc (+) v*...
-//   void   finish(int r, double acc0, double acc1, a0,b0,a1,b1, double *red)
-//                                                    writes rows r, r+1; adds reductions
+//   double  stage(int g)         staged value at extended index g; also what the fused halo
+//                                send stores for a processor-patch face cell
+//   double2 stage_own(int r)     rows r, r+1 of the own band (may also write a fused vector update)
+//   double  init(int r, double a)                 start of the row sum
+//   double  term(double acc, double v, double a)  acc (+) v*a  (default in OpBase: acc + v*a)
+//   void    finish(int r, double acc0, double acc1, double a0, double a1, double *red)
+//                                writes rows r, r+1; adds reductions
 // ---------------------------------------------------------------------------
+
+// Fused halo send (peer-memory path): only operators that stage a vector and read interface
+// entries ever exchange a halo, so the send is compiled for those alone.
+template <class Op>
+__host__ __device__ __forceinline__ bool fused_pack(const Op &op, const LayoutDev &L)
+{
+    return Op::STAGED && !Op::LOCAL && op.waitHalo && L.nPackChunks > 0;
+}
+
 template <class Op>
 __global__ void __launch_bounds__(ENGINE_THREADS, 6) engine_kernel(const LayoutDev L, const double *__restrict__ val, Op op)
 {
-    extern __shared__ double smem[];
+    extern __shared__ double xs[];
     if (!op.prologue(L)) return; // stop flag (OpBase) or the deferred scalar step of the fused PCG (ops.cuh)
-    // Fused halo send (peer-memory path): the first nPackChunks CTAs of the grid gather psi
+    // Fused halo send: the first nPackChunks CTAs of the grid gather the staged vector
     // at the processor-patch face cells, store it straight into the neighbours' receive
     // buffers over NVLink and release their arrival flags; all other CTAs are SpMV bands
     // (those that reference received values wait for the neighbours' flags below).
-    const bool fusedPack = op.waitHalo && L.nPackChunks > 0;
+    const bool fusedPack = fused_pack(op, L);
     unsigned long long haloSeqNow = 0;
     if (fusedPack) {
         haloSeqNow = L.seqs[1] + 1; // seqs[1] only advances when the whole grid has finished
@@ -127,7 +137,7 @@ __global__ void __launch_bounds__(ENGINE_THREADS, 6) engine_kernel(const LayoutD
             const PackPatch P = L.packPatches[c.patch];
             double *dst = P.dst[haloSeqNow & 1];
             for (int i = c.begin + threadIdx.x; i < c.end; i += ENGINE_THREADS)
-                dst[i - P.start] = op.pack_val(__ldg(L.sendRows + i));
+                dst[i - P.start] = op.stage(__ldg(L.sendRows + i));
             __threadfence_system();
             __syncthreads();
             if (threadIdx.x == 0) {
@@ -147,20 +157,13 @@ __global__ void __launch_bounds__(ENGINE_THREADS, 6) engine_kernel(const LayoutD
     }
     const int band = blockIdx.x - (fusedPack ? L.nPackChunks : 0);
     const int rowBase = band * L.bandRows;
-    const int stride = (L.bandRows + L.maxHalo + 1) & ~1; // keep the second tile 16-byte aligned
-    double *xs = smem;
-    double *ys = smem + ((Op::NVEC > 1) ? stride : 0);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     constexpr int NW = ENGINE_THREADS / 32;
 
     // ---- phase 1: stage the band's vector tile + halo ----
-    if (Op::NVEC > 0) {
-    for (int i = tid; i < (L.bandRows >> 1); i += ENGINE_THREADS) {
-        double2 a, b = make_double2(0, 0);
-        op.stage_own(rowBase + 2 * i, a, b);
-        reinterpret_cast<double2 *>(xs)[i] = a;
-        if (Op::NVEC > 1) reinterpret_cast<double2 *>(ys)[i] = b;
-    }
+    if (Op::STAGED) {
+    for (int i = tid; i < (L.bandRows >> 1); i += ENGINE_THREADS)
+        reinterpret_cast<double2 *>(xs)[i] = op.stage_own(rowBase + 2 * i);
     {
         const int hs = L.haloStart[band], hn = L.haloStart[band + 1] - hs;
         // peer-memory halo: bands that reference received values wait for the neighbours'
@@ -176,13 +179,7 @@ __global__ void __launch_bounds__(ENGINE_THREADS, 6) engine_kernel(const LayoutD
         }
         for (int i = tid; i < hn; i += ENGINE_THREADS) {
             int g = __ldg(L.haloIdx + hs + i);
-            double a, b = 0;
-            if (remoteTail && g >= L.nPad)
-                a = __ldcg(remoteTail + (g - L.nPad));
-            else
-                op.stage(g, a, b);
-            xs[L.bandRows + i] = a;
-            if (Op::NVEC > 1) ys[L.bandRows + i] = b;
+            xs[L.bandRows + i] = (remoteTail && g >= L.nPad) ? __ldcg(remoteTail + (g - L.nPad)) : op.stage(g);
         }
     }
     __syncthreads();
@@ -198,10 +195,9 @@ __global__ void __launch_bounds__(ENGINE_THREADS, 6) engine_kernel(const LayoutD
         const long long base = L.sliceStart[s];
         const int W = Op::LOCAL ? L.sliceWL[s] : L.sliceW[s];
         const int lr = sl * SLICE_ROWS + 2 * lane; // local row of this lane's first row
-        const double a0 = (Op::NVEC > 0) ? xs[lr] : 0, a1 = (Op::NVEC > 0) ? xs[lr + 1] : 0;
-        const double b0 = (Op::NVEC > 1) ? ys[lr] : 0, b1 = (Op::NVEC > 1) ? ys[lr + 1] : 0;
-        double acc0 = op.init(rowBase + lr, a0, b0);
-        double acc1 = op.init(rowBase + lr + 1, a1, b1);
+        const double a0 = Op::STAGED ? xs[lr] : 0, a1 = Op::STAGED ? xs[lr + 1] : 0;
+        double acc0 = op.init(rowBase + lr, a0);
+        double acc1 = op.init(rowBase + lr + 1, a1);
         const double *vp = val + base + 2 * lane;
         const uint16_t *cp = L.col + base + 2 * lane;
         int j = 0;
@@ -217,18 +213,18 @@ __global__ void __launch_bounds__(ENGINE_THREADS, 6) engine_kernel(const LayoutD
 #pragma unroll
             for (int k = 0; k < 4; k++) {
                 const int c0 = c[k] & 0xffffu, c1 = c[k] >> 16;
-                acc0 = op.term(acc0, v[k].x, (Op::NVEC > 0) ? xs[c0] : 0, (Op::NVEC > 1) ? ys[c0] : 0);
-                acc1 = op.term(acc1, v[k].y, (Op::NVEC > 0) ? xs[c1] : 0, (Op::NVEC > 1) ? ys[c1] : 0);
+                acc0 = op.term(acc0, v[k].x, Op::STAGED ? xs[c0] : 0);
+                acc1 = op.term(acc1, v[k].y, Op::STAGED ? xs[c1] : 0);
             }
         }
         for (; j < W; j++) {
             double2 v = ldg_stream2(vp + (size_t)j * SLICE_ROWS);
             uint32_t c = ldg_stream_u32(cp + (size_t)j * SLICE_ROWS);
             const int c0 = c & 0xffffu, c1 = c >> 16;
-            acc0 = op.term(acc0, v.x, (Op::NVEC > 0) ? xs[c0] : 0, (Op::NVEC > 1) ? ys[c0] : 0);
-            acc1 = op.term(acc1, v.y, (Op::NVEC > 0) ? xs[c1] : 0, (Op::NVEC > 1) ? ys[c1] : 0);
+            acc0 = op.term(acc0, v.x, Op::STAGED ? xs[c0] : 0);
+            acc1 = op.term(acc1, v.y, Op::STAGED ? xs[c1] : 0);
         }
-        op.finish(rowBase + lr, acc0, acc1, a0, b0, a1, b1, red);
+        op.finish(rowBase + lr, acc0, acc1, a0, a1, red);
     }
     if (Op::NRED > 0) block_reduce_store<(Op::NRED > 0 ? Op::NRED : 1), ENGINE_THREADS>(red, op.partials, band);
     if (fusedPack && threadIdx.x == 0) {
@@ -244,7 +240,7 @@ template <class Op>
 int engine_launch(b200ldu_addr *a, const double *val, const Op &op)
 {
     const LayoutDev &L = a->L;
-    size_t smem = sizeof(double) * (size_t)((L.bandRows + L.maxHalo + 1) & ~1) * (size_t)Op::NVEC;
+    size_t smem = Op::STAGED ? sizeof(double) * (size_t)((L.bandRows + L.maxHalo + 1) & ~1) : 0;
     // the kernel also owns a little static shared memory (reduction scratch): opt in to large dynamic shared
     // memory well before the 48 KB default limit.  The attribute is per device and instantiation.
     static size_t configured[64] = {0};
@@ -253,7 +249,7 @@ int engine_launch(b200ldu_addr *a, const double *val, const Op &op)
         CUDA_TRY(cudaFuncSetAttribute(engine_kernel<Op>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         configured[dev] = smem;
     }
-    int grid = L.nBands + ((op.waitHalo && L.nPackChunks > 0) ? L.nPackChunks : 0);
+    int grid = L.nBands + (fused_pack(op, L) ? L.nPackChunks : 0);
     engine_kernel<Op><<<grid, ENGINE_THREADS, smem, a->ctx->stream>>>(L, val, op);
     a->ctx->launches++;
     KERNEL_CHECK();

@@ -478,34 +478,30 @@ int mat_amul(b200ldu_matrix *m, bool transpose, double *x, double *out, int mode
 {
     int wait = 0;
     TRY(mat_halo(m, x, stop, &wait));
-#define LAUNCH_AMUL(MODE)                  \
-    {                                      \
-        AmulOp<MODE> op;                   \
-        op.stop = stop;                    \
-        op.waitHalo = wait;                \
-        op.partials = partials;            \
-        op.x = x;                          \
-        op.diag = m->d_diag;               \
-        op.aux = aux;                      \
-        op.out = out;                      \
-        return engine_launch_m(m, transpose, op); \
-    }
+    auto launch = [&](auto op) {
+        op.stop = stop;
+        op.waitHalo = wait;
+        op.partials = partials;
+        op.x = x;
+        op.diag = m->d_diag;
+        op.aux = aux;
+        op.out = out;
+        return engine_launch_m(m, transpose, op);
+    };
     switch (mode) {
-    case 0: LAUNCH_AMUL(0)
-    case 1: LAUNCH_AMUL(1)
-    case 2: LAUNCH_AMUL(2)
-    case 3: LAUNCH_AMUL(3)
-    case 4: LAUNCH_AMUL(4)
+    case 0: return launch(AmulOp<0>());
+    case 1: return launch(AmulOp<1>());
+    case 2: return launch(AmulOp<2>());
+    case 3: return launch(AmulOp<3>());
+    case 4: return launch(AmulOp<4>());
     }
-#undef LAUNCH_AMUL
     return B200LDU_EINVAL;
 }
 
 int mat_ainv(b200ldu_matrix *m, bool transpose, const double *r, double *w, bool fuseDot,
              const double *dotv, double *partials, const int *stop)
 {
-    if (fuseDot) {
-        AinvOp<1> op;
+    auto launch = [&](auto op) {
         op.stop = stop;
         op.partials = partials;
         op.r = r;
@@ -513,15 +509,8 @@ int mat_ainv(b200ldu_matrix *m, bool transpose, const double *r, double *w, bool
         op.dotv = dotv;
         op.out = w;
         return engine_launch_m(m, transpose, op);
-    }
-    AinvOp<0> op;
-    op.stop = stop;
-    op.partials = partials;
-    op.r = r;
-    op.rD = m->d_rD;
-    op.dotv = nullptr;
-    op.out = w;
-    return engine_launch_m(m, transpose, op);
+    };
+    return fuseDot ? launch(AinvOp<1>()) : launch(AinvOp<0>());
 }
 
 int mat_jacobi(b200ldu_matrix *m, double omega, double *x, const double *b, double *out, const int *stop)
@@ -536,7 +525,6 @@ int mat_jacobi(b200ldu_matrix *m, double omega, double *x, const double *b, doub
     op.b = b;
     op.out = out;
     op.omega = omega;
-    op.nCells = m->a->nCells;
     return engine_launch_m(m, false, op);
 }
 
@@ -545,8 +533,7 @@ int mat_residual(b200ldu_matrix *m, double *x, const double *b, double *out, boo
 {
     int wait = 0;
     TRY(mat_halo(m, x, stop, &wait));
-    if (fuseSumMag) {
-        ResidualOp<1> op;
+    auto launch = [&](auto op) {
         op.stop = stop;
         op.waitHalo = wait;
         op.partials = partials;
@@ -555,15 +542,8 @@ int mat_residual(b200ldu_matrix *m, double *x, const double *b, double *out, boo
         op.b = b;
         op.out = out;
         return engine_launch_m(m, false, op);
-    }
-    ResidualOp<0> op;
-    op.stop = stop;
-    op.waitHalo = wait;
-    op.x = x;
-    op.diag = m->d_diag;
-    op.b = b;
-    op.out = out;
-    return engine_launch_m(m, false, op);
+    };
+    return fuseSumMag ? launch(ResidualOp<1>()) : launch(ResidualOp<0>());
 }
 
 int mat_sumA(b200ldu_matrix *m, double *out, const int *stop)

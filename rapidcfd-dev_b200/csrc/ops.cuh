@@ -28,6 +28,25 @@ struct OpBase {
     int waitHalo = 0; // 1: a peer-memory halo exchange of the staged vector is in flight
     // first thing every CTA of an engine kernel does; false => the CTA exits (the device has decided to stop)
     __device__ __forceinline__ bool prologue(const LayoutDev &) const { return !(stop && *stop); }
+    // row-sum term acc + v*a; Residual, OffDiag and CoeffSum replace it
+    __device__ __forceinline__ double term(double acc, double v, double a) const
+    {
+        return __dadd_rn(acc, __dmul_rn(v, a));
+    }
+};
+
+// operators that stage the vector x unchanged
+struct StageXOp : OpBase {
+    static constexpr bool STAGED = true;
+    const double *x;
+    __device__ __forceinline__ double stage(int g) const { return x[g]; }
+    __device__ __forceinline__ double2 stage_own(int r) const
+    {
+        // returned as two doubles: a returned double2 lvalue is copied as four 32-bit words, which
+        // renumbers the registers of the staging loop
+        const double2 a = *reinterpret_cast<const double2 *>(x + r);
+        return make_double2(a.x, a.y);
+    }
 };
 
 // ---- Amul / Tmul: out = diag*x + sum v*x[c]  (lduMatrixATmul.C:78-137) ----
@@ -35,28 +54,13 @@ struct OpBase {
 // <source,field>, den = <Acf,field>, GAMGSolverScale.C:80-125];  3: sum(out*aux) [PBiCG
 // wApT, PBiCGStab rA0AyA];  4: sum(out*out), sum(out*aux) [PBiCGStab tAtA, tAsA]
 template <int MODE>
-struct AmulOp : OpBase {
-    static constexpr int NVEC = 1;
+struct AmulOp : StageXOp {
     static constexpr int NRED = (MODE == 0) ? 0 : ((MODE == 1 || MODE == 3) ? 1 : 2);
     static constexpr bool LOCAL = false;
-    const double *x, *diag, *aux;
+    const double *diag, *aux;
     double *out;
-    __device__ __forceinline__ void stage(int g, double &a, double &) const { a = x[g]; }
-    __device__ __forceinline__ double pack_val(int row) const { return x[row]; }
-    __device__ __forceinline__ void stage_own(int r, double2 &a, double2 &) const
-    {
-        a = *reinterpret_cast<const double2 *>(x + r);
-    }
-    __device__ __forceinline__ double init(int r, double a, double) const
-    {
-        return __dmul_rn(diag[r], a);
-    }
-    __device__ __forceinline__ double term(double acc, double v, double a, double) const
-    {
-        return __dadd_rn(acc, __dmul_rn(v, a));
-    }
-    __device__ __forceinline__ void finish(int r, double acc0, double acc1, double a0, double,
-                                           double a1, double, double *red) const
+    __device__ __forceinline__ double init(int r, double a) const { return __dmul_rn(diag[r], a); }
+    __device__ __forceinline__ void finish(int r, double acc0, double acc1, double a0, double a1, double *red) const
     {
         *reinterpret_cast<double2 *>(out + r) = make_double2(acc0, acc1);
         if (MODE == 1) red[0] += acc0 * a0 + acc1 * a1;
@@ -82,25 +86,19 @@ struct AmulOp : OpBase {
 // <w, dotv> (wArA with dotv = r; wArT with dotv = rT).
 template <int NRED_>
 struct AinvOp : OpBase {
-    static constexpr int NVEC = 1, NRED = NRED_;
-    static constexpr bool LOCAL = true;
+    static constexpr bool STAGED = true, LOCAL = true;
+    static constexpr int NRED = NRED_;
     const double *r, *rD, *dotv;
     double *out;
-    __device__ __forceinline__ void stage(int g, double &a, double &) const { a = __dmul_rn(rD[g], r[g]); }
-    __device__ __forceinline__ double pack_val(int) const { return 0.0; }
-    __device__ __forceinline__ void stage_own(int row, double2 &a, double2 &) const
+    __device__ __forceinline__ double stage(int g) const { return __dmul_rn(rD[g], r[g]); }
+    __device__ __forceinline__ double2 stage_own(int row) const
     {
         double2 rr = *reinterpret_cast<const double2 *>(r + row);
         double2 dd = *reinterpret_cast<const double2 *>(rD + row);
-        a = make_double2(__dmul_rn(dd.x, rr.x), __dmul_rn(dd.y, rr.y));
+        return make_double2(__dmul_rn(dd.x, rr.x), __dmul_rn(dd.y, rr.y));
     }
-    __device__ __forceinline__ double init(int, double, double) const { return 0.0; }
-    __device__ __forceinline__ double term(double acc, double v, double t, double) const
-    {
-        return __dadd_rn(acc, __dmul_rn(v, t));
-    }
-    __device__ __forceinline__ void finish(int row, double acc0, double acc1, double, double, double, double,
-                                           double *red) const
+    __device__ __forceinline__ double init(int, double) const { return 0.0; }
+    __device__ __forceinline__ void finish(int row, double acc0, double acc1, double, double, double *red) const
     {
         double2 d = *reinterpret_cast<const double2 *>(rD + row);
         double2 rr = *reinterpret_cast<const double2 *>(r + row);
@@ -115,24 +113,13 @@ struct AinvOp : OpBase {
 };
 
 // ---- Jacobi sweep (JacobiSmootherF.H:51-109; omega-damped, old psi everywhere) ----
-struct JacobiOp : OpBase {
-    static constexpr int NVEC = 1, NRED = 0;
+struct JacobiOp : StageXOp {
+    static constexpr int NRED = 0;
     static constexpr bool LOCAL = false;
-    const double *x, *diag, *b;
+    const double *diag, *b;
     double *out;
     double omega;
-    int nCells;
-    __device__ __forceinline__ void stage(int g, double &a, double &) const { a = x[g]; }
-    __device__ __forceinline__ double pack_val(int row) const { return x[row]; }
-    __device__ __forceinline__ void stage_own(int r, double2 &a, double2 &) const
-    {
-        a = *reinterpret_cast<const double2 *>(x + r);
-    }
-    __device__ __forceinline__ double init(int, double, double) const { return 0.0; }
-    __device__ __forceinline__ double term(double acc, double v, double a, double) const
-    {
-        return __dadd_rn(acc, __dmul_rn(v, a));
-    }
+    __device__ __forceinline__ double init(int, double) const { return 0.0; }
     __device__ __forceinline__ double row(int r, double acc, double a) const
     {
         double rD = __ddiv_rn(1.0, diag[r]);
@@ -140,8 +127,7 @@ struct JacobiOp : OpBase {
         double extra = __dadd_rn(__dmul_rn(1 - omega, a), __dmul_rn(w, b[r]));
         return __dsub_rn(extra, __dmul_rn(w, acc));
     }
-    __device__ __forceinline__ void finish(int r, double acc0, double acc1, double a0, double,
-                                           double a1, double, double *) const
+    __device__ __forceinline__ void finish(int r, double acc0, double acc1, double a0, double a1, double *) const
     {
         *reinterpret_cast<double2 *>(out + r) = make_double2(row(r, acc0, a0), row(r + 1, acc1, a1));
     }
@@ -149,27 +135,17 @@ struct JacobiOp : OpBase {
 
 // ---- residual: rA = (b - diag*x) - sum v*x ; fused sum|rA|  (lduMatrixATmul.C:397-496)
 template <int NRED_>
-struct ResidualOp : OpBase {
-    static constexpr int NVEC = 1, NRED = NRED_;
+struct ResidualOp : StageXOp {
+    static constexpr int NRED = NRED_;
     static constexpr bool LOCAL = false;
-    const double *x, *diag, *b;
+    const double *diag, *b;
     double *out;
-    __device__ __forceinline__ void stage(int g, double &a, double &) const { a = x[g]; }
-    __device__ __forceinline__ double pack_val(int row) const { return x[row]; }
-    __device__ __forceinline__ void stage_own(int r, double2 &a, double2 &) const
-    {
-        a = *reinterpret_cast<const double2 *>(x + r);
-    }
-    __device__ __forceinline__ double init(int r, double a, double) const
-    {
-        return __dsub_rn(b[r], __dmul_rn(diag[r], a));
-    }
-    __device__ __forceinline__ double term(double acc, double v, double a, double) const
+    __device__ __forceinline__ double init(int r, double a) const { return __dsub_rn(b[r], __dmul_rn(diag[r], a)); }
+    __device__ __forceinline__ double term(double acc, double v, double a) const
     {
         return __dsub_rn(acc, __dmul_rn(v, a));
     }
-    __device__ __forceinline__ void finish(int r, double acc0, double acc1, double, double, double,
-                                           double, double *red) const
+    __device__ __forceinline__ void finish(int r, double acc0, double acc1, double, double, double *red) const
     {
         *reinterpret_cast<double2 *>(out + r) = make_double2(acc0, acc1);
         if (NRED == 1) red[0] += fabs(acc0) + fabs(acc1);
@@ -179,23 +155,18 @@ struct ResidualOp : OpBase {
 // ---- coefficient-only row sums: sumA (all entries, + diag), H1 (local, negated) ----
 template <bool LOCAL_, bool NEG_>
 struct CoeffSumOp : OpBase {
-    static constexpr int NVEC = 0, NRED = 0;
-    static constexpr bool LOCAL = LOCAL_;
+    static constexpr bool STAGED = false, LOCAL = LOCAL_;
+    static constexpr int NRED = 0;
     const double *diag; // nullptr => start from 0
     double *out;
-    __device__ __forceinline__ void stage(int, double &, double &) const {}
-    __device__ __forceinline__ double pack_val(int) const { return 0.0; }
-    __device__ __forceinline__ void stage_own(int, double2 &, double2 &) const {}
-    __device__ __forceinline__ double init(int r, double, double) const
-    {
-        return diag ? diag[r] : 0.0;
-    }
-    __device__ __forceinline__ double term(double acc, double v, double, double) const
+    __device__ __forceinline__ double stage(int) const { return 0.0; }
+    __device__ __forceinline__ double2 stage_own(int) const { return make_double2(0, 0); }
+    __device__ __forceinline__ double init(int r, double) const { return diag ? diag[r] : 0.0; }
+    __device__ __forceinline__ double term(double acc, double v, double) const
     {
         return NEG_ ? __dsub_rn(acc, v) : __dadd_rn(acc, v);
     }
-    __device__ __forceinline__ void finish(int r, double acc0, double acc1, double, double, double,
-                                           double, double *) const
+    __device__ __forceinline__ void finish(int r, double acc0, double acc1, double, double, double *) const
     {
         *reinterpret_cast<double2 *>(out + r) = make_double2(acc0, acc1);
     }
@@ -204,24 +175,17 @@ struct CoeffSumOp : OpBase {
 // ---- off-diagonal product sums: H = -(sum v*x) local only (lduMatrixOperations.C:107-155);
 // GAMG interpolate: psi' = -(sum v*x)/diag over all entries (GAMGSolverInterpolate.C:45-110)
 template <bool LOCAL_, bool DIVDIAG_>
-struct OffDiagOp : OpBase {
-    static constexpr int NVEC = 1, NRED = 0;
+struct OffDiagOp : StageXOp {
+    static constexpr int NRED = 0;
     static constexpr bool LOCAL = LOCAL_;
-    const double *x, *diag;
+    const double *diag;
     double *out;
-    __device__ __forceinline__ void stage(int g, double &a, double &) const { a = x[g]; }
-    __device__ __forceinline__ double pack_val(int row) const { return x[row]; }
-    __device__ __forceinline__ void stage_own(int r, double2 &a, double2 &) const
+    __device__ __forceinline__ double init(int, double) const { return 0.0; }
+    __device__ __forceinline__ double term(double acc, double v, double a) const
     {
-        a = *reinterpret_cast<const double2 *>(x + r);
+        return DIVDIAG_ ? OpBase::term(acc, v, a) : __dsub_rn(acc, __dmul_rn(v, a));
     }
-    __device__ __forceinline__ double init(int, double, double) const { return 0.0; }
-    __device__ __forceinline__ double term(double acc, double v, double a, double) const
-    {
-        return DIVDIAG_ ? __dadd_rn(acc, __dmul_rn(v, a)) : __dsub_rn(acc, __dmul_rn(v, a));
-    }
-    __device__ __forceinline__ void finish(int r, double acc0, double acc1, double, double, double,
-                                           double, double *) const
+    __device__ __forceinline__ void finish(int r, double acc0, double acc1, double, double, double *) const
     {
         if (DIVDIAG_) {
             acc0 = __ddiv_rn(-acc0, diag[r]);
@@ -439,20 +403,19 @@ struct DeferredStep {
 // read the old halo values), psi is updated in place (own rows only).
 template <class Pre>
 struct PcgAinvOp : OpBase {
-    static constexpr int NVEC = 1, NRED = 2;
-    static constexpr bool LOCAL = true;
+    static constexpr bool STAGED = true, LOCAL = true;
+    static constexpr int NRED = 2;
     const double *rOld, *w, *p, *rD;
     double *rNew, *psi, *z;
     const SolverScalars *sc;
     Pre pre; // scalar step of the previous sweep, run in this kernel's prologue
     __device__ __forceinline__ bool prologue(const LayoutDev &) const { return pre.run(); }
-    __device__ __forceinline__ void stage(int g, double &a, double &) const
+    __device__ __forceinline__ double stage(int g) const
     {
         double r = sc->bodies > 0 ? fma(-sc->alpha, w[g], rOld[g]) : rOld[g];
-        a = __dmul_rn(rD[g], r);
+        return __dmul_rn(rD[g], r);
     }
-    __device__ __forceinline__ double pack_val(int) const { return 0.0; }
-    __device__ __forceinline__ void stage_own(int row, double2 &a, double2 &) const
+    __device__ __forceinline__ double2 stage_own(int row) const
     {
         double2 r = *reinterpret_cast<const double2 *>(rOld + row);
         if (sc->bodies > 0) {
@@ -468,15 +431,10 @@ struct PcgAinvOp : OpBase {
         }
         *reinterpret_cast<double2 *>(rNew + row) = r;
         double2 dd = *reinterpret_cast<const double2 *>(rD + row);
-        a = make_double2(__dmul_rn(dd.x, r.x), __dmul_rn(dd.y, r.y));
+        return make_double2(__dmul_rn(dd.x, r.x), __dmul_rn(dd.y, r.y));
     }
-    __device__ __forceinline__ double init(int, double, double) const { return 0.0; }
-    __device__ __forceinline__ double term(double acc, double v, double t, double) const
-    {
-        return __dadd_rn(acc, __dmul_rn(v, t));
-    }
-    __device__ __forceinline__ void finish(int row, double acc0, double acc1, double, double, double, double,
-                                           double *red) const
+    __device__ __forceinline__ double init(int, double) const { return 0.0; }
+    __device__ __forceinline__ void finish(int row, double acc0, double acc1, double, double, double *red) const
     {
         // rNew[row] was written by this CTA in phase 1 (visible after the barrier)
         double2 d = *reinterpret_cast<const double2 *>(rD + row);
@@ -490,24 +448,21 @@ struct PcgAinvOp : OpBase {
 };
 
 // K_B: forms the new search direction while staging (p = z on the first body, else
-// z + beta p; beta from the device scalars; p ping-ponged), w = A p, fused <w,p>.  The halo
-// send (fused pack CTAs) evaluates the same expression at the patch face cells.
+// z + beta p; beta from the device scalars; p ping-ponged), then the row arithmetic of
+// AmulOp<1>: w = A p, fused <w,p>.  The halo send (fused pack CTAs) stages the same p at
+// the patch face cells.
 template <class Pre>
-struct PcgAmulOp : OpBase {
-    static constexpr int NVEC = 1, NRED = 1;
-    static constexpr bool LOCAL = false;
-    const double *z, *pOld, *diag;
-    double *pNew, *out;
+struct PcgAmulOp : AmulOp<1> {
+    const double *z, *pOld;
+    double *pNew;
     const SolverScalars *sc;
     Pre pre; // scalar step of the previous sweep, run in this kernel's prologue
     __device__ __forceinline__ bool prologue(const LayoutDev &) const { return pre.run(); }
-    __device__ __forceinline__ double pval(int g) const
+    __device__ __forceinline__ double stage(int g) const
     {
         return sc->bodies == 0 ? z[g] : fma(sc->beta, pOld[g], z[g]);
     }
-    __device__ __forceinline__ void stage(int g, double &a, double &) const { a = pval(g); }
-    __device__ __forceinline__ double pack_val(int row) const { return pval(row); }
-    __device__ __forceinline__ void stage_own(int row, double2 &a, double2 &) const
+    __device__ __forceinline__ double2 stage_own(int row) const
     {
         double2 zz = *reinterpret_cast<const double2 *>(z + row);
         if (sc->bodies > 0) {
@@ -517,17 +472,6 @@ struct PcgAmulOp : OpBase {
             zz.y = fma(beta, po.y, zz.y);
         }
         *reinterpret_cast<double2 *>(pNew + row) = zz;
-        a = zz;
-    }
-    __device__ __forceinline__ double init(int r, double a, double) const { return __dmul_rn(diag[r], a); }
-    __device__ __forceinline__ double term(double acc, double v, double a, double) const
-    {
-        return __dadd_rn(acc, __dmul_rn(v, a));
-    }
-    __device__ __forceinline__ void finish(int r, double acc0, double acc1, double a0, double, double a1,
-                                           double, double *red) const
-    {
-        *reinterpret_cast<double2 *>(out + r) = make_double2(acc0, acc1);
-        red[0] += acc0 * a0 + acc1 * a1;
+        return zz;
     }
 };

@@ -310,7 +310,7 @@ int solve_pcg_fused(Solve &S, int pk)
         int wait = 0;
         TRY(mat_halo(m, pNew, stop, &wait)); // peer-memory path: nothing is launched, the send is fused
         const PreB preB{partA, npA, sc, gA, pr, (unsigned)(2 * (k % every) + 1), mod, 1};
-        PcgAmulOp<PreB> op;
+        PcgAmulOp<PreB> op{}; // zeroes the x and aux it inherits from AmulOp<1> and does not read
         op.stop = stop;
         op.partials = partB;
         op.waitHalo = wait;
