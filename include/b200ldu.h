@@ -114,6 +114,10 @@ int b200ldu_addr_destroy(b200ldu_addr *a);
 /* introspection (tests, DESIGN.md numbers) */
 int b200ldu_addr_info(const b200ldu_addr *a, long long *nPadRows, long long *nEntries,
                       long long *nHalo, int *bandRows, int *nBands);
+/* face stream of symmetric matrices: stored owner slots (padding included), list items, product-buffer doubles
+ * of the largest band, and whether symmetric matrices on this addressing use it (1) or the entry stream (0) */
+int b200ldu_addr_face_info(const b200ldu_addr *a, long long *nOwnerSlots, long long *nListItems, int *bufDoubles,
+                           int *used);
 /* cell renumbering: perm_h[c] = banded row of caller cell c (HOST int32[nCells]) */
 int b200ldu_addr_perm(const b200ldu_addr *a, int *perm_h);
 

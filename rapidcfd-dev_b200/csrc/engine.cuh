@@ -106,9 +106,18 @@ __device__ __forceinline__ void block_reduce_store(double (&red)[NRED], double *
 //                                send stores for a processor-patch face cell
 //   double2 stage_own(int r)     rows r, r+1 of the own band (may also write a fused vector update)
 //   double  init(int r, double a)                 start of the row sum
-//   double  term(double acc, double v, double a)  acc (+) v*a  (default in OpBase: acc + v*a)
+//   double  prod(double v, double a)              the term of coefficient v and staged value a (default v*a)
+//   double  add(double acc, double p)             adds a term to the row sum (default acc + p)
+//   double  identity()                            p with add(acc, p) == acc bit for bit (default -0.0)
 //   void    finish(int r, double acc0, double acc1, double a0, double a1, double *red)
 //                                writes rows r, r+1; adds reductions
+//
+// Face stream (FS, symmetric matrices; layout.cu): the band's product buffer follows the tile in shared memory and
+// starts filled with identity().  Pass 1 streams the owner slots of each row: add(init, owner terms) in face order,
+// stored in the row's slot 0, while every owner entry whose neighbour row lies in the band stores prod(v, a_own) in
+// that row's neighbour slot; the CTA then stores the products of the band's list (faces owned in other bands,
+// coupled-patch faces).  After one barrier pass 2 adds each row's slots in order -- neighbour faces in losort order,
+// then interface faces -- so every row sum is the entry stream's, operation for operation.
 // ---------------------------------------------------------------------------
 
 // Fused halo send (peer-memory path): only operators that stage a vector and read interface
@@ -119,7 +128,25 @@ __host__ __device__ __forceinline__ bool fused_pack(const Op &op, const LayoutDe
     return Op::STAGED && !Op::LOCAL && op.waitHalo && L.nPackChunks > 0;
 }
 
+__device__ __forceinline__ uint2 ldg_stream_u64(const void *p)
+{
+    uint2 r;
+    asm volatile("ld.global.nc.L1::no_allocate.v2.u32 {%0, %1}, [%2];" : "=r"(r.x), "=r"(r.y) : "l"(p));
+    return r;
+}
+
+// one owner entry of the face stream: ct = column | product slot << 16
 template <class Op>
+__device__ __forceinline__ double fs_owner(const Op &op, const double *xs, double *buf, double acc, double v,
+                                           uint32_t ct, double aOwn)
+{
+    const uint32_t c = ct & 0xffffu, t = ct >> 16;
+    if (t != FS_PAD) acc = op.add(acc, op.prod(v, Op::STAGED ? xs[c] : 0));
+    if (t < FS_PAD) buf[t] = op.prod(v, aOwn);
+    return acc;
+}
+
+template <class Op, bool FS>
 __global__ void __launch_bounds__(ENGINE_THREADS, 6) engine_kernel(const LayoutDev L, const double *__restrict__ val, Op op)
 {
     extern __shared__ double xs[];
@@ -161,6 +188,7 @@ __global__ void __launch_bounds__(ENGINE_THREADS, 6) engine_kernel(const LayoutD
     constexpr int NW = ENGINE_THREADS / 32;
 
     // ---- phase 1: stage the band's vector tile + halo ----
+    double *const buf = xs + (Op::STAGED ? ((L.bandRows + L.maxHalo + 1) & ~1) : 0); // face stream: product buffer
     if (Op::STAGED) {
     for (int i = tid; i < (L.bandRows >> 1); i += ENGINE_THREADS)
         reinterpret_cast<double2 *>(xs)[i] = op.stage_own(rowBase + 2 * i);
@@ -182,14 +210,79 @@ __global__ void __launch_bounds__(ENGINE_THREADS, 6) engine_kernel(const LayoutD
             xs[L.bandRows + i] = (remoteTail && g >= L.nPad) ? __ldcg(remoteTail + (g - L.nPad)) : op.stage(g);
         }
     }
-    __syncthreads();
     }
+    if (FS) {
+        const double e = op.identity();
+        for (int i = tid; i < (L.fsBufMax >> 1); i += ENGINE_THREADS) reinterpret_cast<double2 *>(buf)[i] = make_double2(e, e);
+    }
+    if (Op::STAGED || FS) __syncthreads();
 
     // ---- phase 2: row sums ----
     double red[Op::NRED > 0 ? Op::NRED : 1];
 #pragma unroll
     for (int k = 0; k < (Op::NRED > 0 ? Op::NRED : 1); k++) red[k] = 0;
 
+    if constexpr (FS) {
+        // pass 1: owner slots, then the band's list
+        for (int sl = warp; sl < L.slicesPerBand; sl += NW) {
+            const FsSlice S = L.fsSlice[band * L.slicesPerBand + sl];
+            const int lr = sl * SLICE_ROWS + 2 * lane;
+            const double a0 = Op::STAGED ? xs[lr] : 0, a1 = Op::STAGED ? xs[lr + 1] : 0;
+            double acc0 = op.init(rowBase + lr, a0);
+            double acc1 = op.init(rowBase + lr + 1, a1);
+            const long long base = (long long)S.start64 * SLICE_ROWS + 2 * lane;
+            const double *vp = val + base;
+            const uint32_t *cp = L.fsCT + base;
+            const int W = S.wo;
+            int j = 0;
+            for (; j + 4 <= W; j += 4) {
+                double2 v[4];
+                uint2 c[4];
+#pragma unroll
+                for (int k = 0; k < 4; k++) {
+                    v[k] = ldg_stream2(vp + (size_t)(j + k) * SLICE_ROWS);
+                    c[k] = ldg_stream_u64(cp + (size_t)(j + k) * SLICE_ROWS);
+                }
+#pragma unroll
+                for (int k = 0; k < 4; k++) {
+                    acc0 = fs_owner(op, xs, buf, acc0, v[k].x, c[k].x, a0);
+                    acc1 = fs_owner(op, xs, buf, acc1, v[k].y, c[k].y, a1);
+                }
+            }
+            for (; j < W; j++) {
+                double2 v = ldg_stream2(vp + (size_t)j * SLICE_ROWS);
+                uint2 c = ldg_stream_u64(cp + (size_t)j * SLICE_ROWS);
+                acc0 = fs_owner(op, xs, buf, acc0, v.x, c.x, a0);
+                acc1 = fs_owner(op, xs, buf, acc1, v.y, c.y, a1);
+            }
+            reinterpret_cast<double2 *>(buf + S.bufOff)[lane] = make_double2(acc0, acc1);
+        }
+        {
+            const int le = Op::LOCAL ? L.fsListIfc[band] : L.fsListStart[band + 1];
+            for (int i = L.fsListStart[band] + tid; i < le; i += ENGINE_THREADS) {
+                const double v = __ldcs(val + i);
+                const uint32_t ct = __ldcs(L.fsCT + i);
+                buf[ct >> 16] = op.prod(v, Op::STAGED ? xs[ct & 0xffffu] : 0);
+            }
+        }
+        __syncthreads();
+        // pass 2: each row's sum, then its buffer slots in order
+        for (int sl = warp; sl < L.slicesPerBand; sl += NW) {
+            const FsSlice S = L.fsSlice[band * L.slicesPerBand + sl];
+            const int lr = sl * SLICE_ROWS + 2 * lane;
+            const double2 *bp = reinterpret_cast<const double2 *>(buf + S.bufOff) + lane;
+            const double2 s0 = bp[0];
+            double acc0 = s0.x, acc1 = s0.y;
+            const int W = 1 + S.wn + (Op::LOCAL ? 0 : S.wi);
+            for (int j = 1; j < W; j++) {
+                const double2 p = bp[j * (SLICE_ROWS / 2)];
+                acc0 = op.add(acc0, p.x);
+                acc1 = op.add(acc1, p.y);
+            }
+            const double a0 = Op::STAGED ? xs[lr] : 0, a1 = Op::STAGED ? xs[lr + 1] : 0;
+            op.finish(rowBase + lr, acc0, acc1, a0, a1, red);
+        }
+    } else
     for (int sl = warp; sl < L.slicesPerBand; sl += NW) {
         const int s = band * L.slicesPerBand + sl;
         const long long base = L.sliceStart[s];
@@ -213,16 +306,16 @@ __global__ void __launch_bounds__(ENGINE_THREADS, 6) engine_kernel(const LayoutD
 #pragma unroll
             for (int k = 0; k < 4; k++) {
                 const int c0 = c[k] & 0xffffu, c1 = c[k] >> 16;
-                acc0 = op.term(acc0, v[k].x, Op::STAGED ? xs[c0] : 0);
-                acc1 = op.term(acc1, v[k].y, Op::STAGED ? xs[c1] : 0);
+                acc0 = op.add(acc0, op.prod(v[k].x, Op::STAGED ? xs[c0] : 0));
+                acc1 = op.add(acc1, op.prod(v[k].y, Op::STAGED ? xs[c1] : 0));
             }
         }
         for (; j < W; j++) {
             double2 v = ldg_stream2(vp + (size_t)j * SLICE_ROWS);
             uint32_t c = ldg_stream_u32(cp + (size_t)j * SLICE_ROWS);
             const int c0 = c & 0xffffu, c1 = c >> 16;
-            acc0 = op.term(acc0, v.x, Op::STAGED ? xs[c0] : 0);
-            acc1 = op.term(acc1, v.y, Op::STAGED ? xs[c1] : 0);
+            acc0 = op.add(acc0, op.prod(v.x, Op::STAGED ? xs[c0] : 0));
+            acc1 = op.add(acc1, op.prod(v.y, Op::STAGED ? xs[c1] : 0));
         }
         op.finish(rowBase + lr, acc0, acc1, a0, a1, red);
     }
@@ -236,29 +329,30 @@ __global__ void __launch_bounds__(ENGINE_THREADS, 6) engine_kernel(const LayoutD
     }
 }
 
-template <class Op>
+template <class Op, bool FS>
 int engine_launch(b200ldu_addr *a, const double *val, const Op &op)
 {
     const LayoutDev &L = a->L;
-    size_t smem = Op::STAGED ? sizeof(double) * (size_t)((L.bandRows + L.maxHalo + 1) & ~1) : 0;
+    size_t smem = sizeof(double) * ((Op::STAGED ? (size_t)((L.bandRows + L.maxHalo + 1) & ~1) : 0) + (FS ? (size_t)L.fsBufMax : 0));
     // the kernel also owns a little static shared memory (reduction scratch): opt in to large dynamic shared
     // memory well before the 48 KB default limit.  The attribute is per device and instantiation.
     static size_t configured[64] = {0};
     const int dev = a->ctx->device & 63;
     if (smem > 40 * 1024 && smem > configured[dev]) {
-        CUDA_TRY(cudaFuncSetAttribute(engine_kernel<Op>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        CUDA_TRY(cudaFuncSetAttribute(engine_kernel<Op, FS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         configured[dev] = smem;
     }
     int grid = L.nBands + (fused_pack(op, L) ? L.nPackChunks : 0);
-    engine_kernel<Op><<<grid, ENGINE_THREADS, smem, a->ctx->stream>>>(L, val, op);
+    engine_kernel<Op, FS><<<grid, ENGINE_THREADS, smem, a->ctx->stream>>>(L, val, op);
     a->ctx->launches++;
     KERNEL_CHECK();
     return B200LDU_OK;
 }
 
-// matrix sweep with A's coefficients, or A^T's
+// matrix sweep with A's coefficients, or A^T's: a symmetric matrix streams its faces once (A == A^T)
 template <class Op>
 int engine_launch_m(b200ldu_matrix *m, bool transpose, const Op &op)
 {
-    return engine_launch(m->a, transpose ? m->d_valT : m->d_val, op);
+    if (m->d_fval) return engine_launch<Op, true>(m->a, m->d_fval, op);
+    return engine_launch<Op, false>(m->a, transpose ? m->d_valT : m->d_val, op);
 }

@@ -94,6 +94,19 @@ struct PackChunk {
     int patch, begin, end;
 };
 
+// Face stream of a symmetric matrix (layout.cu, engine.cuh): every face is stored once, in its owner's row; the
+// product for the neighbour's row goes through a per-band shared-memory buffer.  Per slice of 64 rows:
+struct FsSlice {
+    int start64;      // owner-stream offset of the slice / 64
+    int bufOff;       // offset of the slice's product slots in the band's buffer (doubles)
+    uint16_t wo;      // owner slots per row
+    uint16_t wn, wi;  // buffer slots per row after slot 0 (the owner-pass sum): neighbour faces, then interface faces
+    uint16_t unused;
+};
+// 16-bit product-slot value of an owner entry: a buffer index, or one of these
+constexpr uint32_t FS_PAD = 0xfffe;  // padding entry: contributes nothing
+constexpr uint32_t FS_NONE = 0xffff; // the neighbour row lies in another band (its band's list carries the product)
+
 // device view of the banded addressing, passed by value to kernels
 struct LayoutDev {
     int nCells;         // real rows
@@ -109,6 +122,13 @@ struct LayoutDev {
     const uint16_t *col;         // [nEntries] band-local column: < bandRows own band, else halo slot
     const int *haloStart;        // [nBands+1]
     const int *haloIdx;          // banded extended index: < nPad local row, else nPad + recv slot
+    // face stream (null when the layout has none): entries [0, nOwn) are the slot-major owner stream, then the
+    // per-band lists; each entry's word is column | product slot << 16
+    const FsSlice *fsSlice;      // [nSlices]
+    const uint32_t *fsCT;        // [nOwn + nList]
+    const int *fsListStart;      // [nBands+1] list of band b: [fsListStart[b], fsListIfc[b]) faces whose owner row
+    const int *fsListIfc;        // [nBands]   lies in another band, then coupled-patch faces up to fsListStart[b+1]
+    int fsBufMax;                // product-buffer doubles of the largest band
     const int *perm;             // [nCells] caller cell -> banded row
     const int *iperm;            // [nPad]  banded row -> caller cell, -1 padding
     // peer-memory halo (null/0 when the exchange goes through NCCL into the vector's own tail)
@@ -140,6 +160,13 @@ struct b200ldu_addr {
     long long *d_sliceStart = nullptr;
     uint16_t *d_sliceW = nullptr, *d_sliceWL = nullptr, *d_col = nullptr;
     int *d_code = nullptr; // [nEntries] value source: 2f+side | -1 pad | -2-pf interface
+    // face stream: used by symmetric matrices when the layout has one (hasFs)
+    bool hasFs = false;
+    long long fsOwn = 0, fsList = 0; // stored owner slots (padding included), list items
+    FsSlice *d_fsSlice = nullptr;
+    uint32_t *d_fsCT = nullptr;
+    int *d_fsCode = nullptr; // [fsOwn + fsList] value source, as d_code
+    int *d_fsListStart = nullptr, *d_fsListIfc = nullptr;
     int *d_haloStart = nullptr, *d_haloIdx = nullptr, *d_perm = nullptr, *d_iperm = nullptr;
     int *d_sendRows = nullptr; // [nRecv] banded row of faceCells (pack kernel)
     bool p2pHalo = false;      // peer-store halo usable for this addressing
@@ -167,6 +194,9 @@ struct b200ldu_addr {
     std::vector<long long> dbg_sliceStart;
     std::vector<uint16_t> dbg_sliceW, dbg_sliceWL, dbg_col;
     std::vector<int> dbg_code, dbg_haloStart, dbg_haloIdx;
+    std::vector<FsSlice> dbg_fsSlice;
+    std::vector<uint32_t> dbg_fsCT;
+    std::vector<int> dbg_fsCode, dbg_fsListStart, dbg_fsListIfc;
     // workspace pool for caller-order entry points (banded vectors)
     std::vector<double *> pool;
     long long vecLen = 0; // nPad + nRecv (padded to even)
@@ -178,6 +208,7 @@ struct b200ldu_matrix {
     bool haveT = false;
     double *d_val = nullptr;  // banded coefficients for Amul   [nEntries]
     double *d_valT = nullptr; // banded coefficients for Tmul   (aliases d_val when symmetric)
+    double *d_fval = nullptr; // face-stream coefficients [fsOwn + fsList]: a symmetric matrix has these instead of d_val
     double *d_diag = nullptr; // banded diagonal [nPad] (padding rows = 1)
     double *d_rD = nullptr;   // 1/diag, filled by matrix_set
     // caller-order coefficients OWNED by the matrix (copied by matrix_set): diag, upper, lower, interfaceBouCoeffs,

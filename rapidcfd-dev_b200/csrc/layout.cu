@@ -124,9 +124,15 @@ int pick_band_rows(int nCells, int smCount, int packCtas)
     // A mesh that fits one wave is best served by exactly one (every CTA resident at once, fewer partial sums for
     // the scalar step).  Beyond that, whole waves are the WORST choice -- the CTAs of a wave stage and stream in lock-step, so the
     // SM alternates between a latency-bound and a bandwidth-bound phase -- and 4+ waves of smaller bands, which drift out of
-    // phase, are best; the bands grow to 1024 rows as the mesh allows.  At 256^3 a 1024-row band's sweep A (the AINV
-    // sweep, whose staging phase carries most of its vector bytes) takes 782 us against 849 us for 2048 rows; sweep B
-    // 583 against 597 us (torch.profiler, bench_kernels.py --pcg-sweeps): 20 waves drift apart better than 10.
+    // phase, are best.  At 256^3 a 1024-row band's sweep A (the AINV sweep, whose staging phase carries most of its
+    // vector bytes) takes 782 us against 849 us for 2048 rows; sweep B 583 against 597 us (torch.profiler,
+    // bench_kernels.py --pcg-sweeps): 20 waves drift apart better than 10.
+    // The bands grow to 512 rows as the mesh allows: there the face stream of symmetric matrices (tile + product buffer,
+    // ~23 KB) keeps 6 CTAs per SM, at 1024 rows (~46 KB) only 4.  Measured on one H100 80GB HBM3 at a 400 W power
+    // limit, 256^3, bench.py --steps 5, three alternating runs each: 512 rows + face stream (this rule) 12.44-12.51 k |
+    // 1024 rows + face stream 11.88-11.89 k | 1024 rows, entry stream (the previous rule) 11.23-11.27 k.  The
+    // asymmetric PBiCG leg, which keeps the entry stream, loses 1.4 % to the narrower bands (5.57-5.58 k against
+    // 5.65-5.66 k).
     // the packing CTAs of the fused halo send share the grid with the bands: keep bands + packers within the one wave
     const long long slots = (long long)(smCount > 0 ? smCount : 132) * 6 - packCtas;
     const long long maxRows = 2432; // the tile of a band + its halo must leave room for 6 CTAs per SM
@@ -137,8 +143,16 @@ int pick_band_rows(int nCells, int smCount, int packCtas)
     }
     const long long target = nCells / (slots * 4);
     int b = SLICE_ROWS;
-    while (b * 2 <= target && b < 1024) b *= 2;
+    while (b * 2 <= target && b < 512) b *= 2;
     return b;
+}
+
+// resident engine CTAs per SM for a band's dynamic shared memory: 228 KB per SM, 1 KB of it reserved per CTA and
+// about 1 KB of static scratch; the 40-register budget allows 6
+int ctas_per_sm(long long smemDoubles)
+{
+    const long long per = smemDoubles * (long long)sizeof(double) + 2048;
+    return (int)std::min<long long>(6, 228 * 1024 / per);
 }
 
 } // namespace
@@ -294,6 +308,65 @@ int layout_build(b200ldu_addr *a, const double *centres)
         sliceStart[s + 1] = sliceStart[s] + (long long)sliceW[s] * SLICE_ROWS;
     const long long nEntries = sliceStart[nSlices];
 
+    // ---- 2b. face stream: slice widths, product-buffer offsets, list sizes ----
+    // nbSlot[f]: position of face f among its neighbour cell's losort faces
+    std::vector<int> nbSlot((size_t)std::max(nFaces, 1));
+    for (int c = 0; c < nCells; c++)
+        for (int k = losortStart[c]; k < losortStart[c + 1]; k++) nbSlot[losort[k]] = k - losortStart[c];
+    std::vector<FsSlice> fsSlice(nSlices);
+#pragma omp parallel for schedule(static)
+    for (int s = 0; s < nSlices; s++) {
+        int wo = 0, wn = 0, wi = 0;
+        for (int q = 0; q < SLICE_ROWS; q++) {
+            int c = iperm[(size_t)s * SLICE_ROWS + q];
+            if (c < 0) continue;
+            wo = std::max(wo, ownerStart[c + 1] - ownerStart[c]);
+            wn = std::max(wn, losortStart[c + 1] - losortStart[c]);
+            wi = std::max(wi, pfStart[c + 1] - pfStart[c]);
+        }
+        fsSlice[s] = FsSlice{0, 0, (uint16_t)wo, (uint16_t)wn, (uint16_t)wi, 0};
+    }
+    long long fsBufMax = 0, fsOwn = 0;
+    for (int b = 0; b < nBands; b++) {
+        long long off = 0;
+        for (int sl = 0; sl < slicesPerBand; sl++) {
+            FsSlice &S = fsSlice[(size_t)b * slicesPerBand + sl];
+            S.start64 = (int)(fsOwn / SLICE_ROWS);
+            S.bufOff = (int)std::min<long long>(off, INT32_MAX);
+            fsOwn += (long long)S.wo * SLICE_ROWS;
+            off += (1 + (long long)S.wn + S.wi) * SLICE_ROWS;
+        }
+        fsBufMax = std::max(fsBufMax, off);
+    }
+    std::vector<int> fsListStart((size_t)nBands + 1, 0), fsListIfc(nBands, 0); // counts first
+#pragma omp parallel for schedule(static)
+    for (int b = 0; b < nBands; b++) {
+        const int r0 = b * bandRows, r1 = r0 + bandRows;
+        int nx = 0, ni = 0;
+        for (int r = r0; r < r1; r++) {
+            int c = iperm[r];
+            if (c < 0) continue;
+            for (int k = losortStart[c]; k < losortStart[c + 1]; k++) {
+                int t = perm[l[losort[k]]];
+                nx += (t < r0 || t >= r1);
+            }
+            ni += pfStart[c + 1] - pfStart[c];
+        }
+        fsListIfc[b] = nx;
+        fsListStart[b + 1] = nx + ni;
+    }
+    fsListStart[0] = (int)std::min<long long>(fsOwn, INT32_MAX);
+    for (int b = 0; b < nBands; b++) {
+        const long long next = (long long)fsListStart[b] + fsListStart[b + 1];
+        fsListIfc[b] += fsListStart[b];
+        fsListStart[b + 1] = (int)std::min<long long>(next, INT32_MAX);
+    }
+    const long long fsList = (long long)fsListStart[nBands] - fsListStart[0];
+    // the 16-bit product slots must address the whole buffer, the 32-bit stream offsets every entry
+    bool fsFits = fsBufMax < (long long)FS_PAD && fsOwn + fsList < INT32_MAX;
+    std::vector<uint32_t> fsCT(fsFits ? (size_t)std::max<long long>(fsOwn + fsList, 1) : 1);
+    std::vector<int> fsCode(fsCT.size());
+
     // ---- 3. per-band halo lists and entries ---------------------------------
     std::vector<uint16_t> col((size_t)std::max<long long>(nEntries, 1));
     std::vector<int> code((size_t)std::max<long long>(nEntries, 1));
@@ -363,6 +436,49 @@ int layout_build(b200ldu_addr *a, const double *centres)
                 }
             }
         }
+        if (!fsFits) continue;
+        // face stream: product slot j of row n (slot 0 holds the row's owner-pass sum)
+        auto slotOf = [&](int n, int j) -> uint32_t {
+            const FsSlice &S = fsSlice[n / SLICE_ROWS];
+            return (uint32_t)(S.bufOff + j * SLICE_ROWS + n % SLICE_ROWS);
+        };
+        for (int sl = 0; sl < slicesPerBand; sl++) {
+            const int s = b * slicesPerBand + sl;
+            const FsSlice &S = fsSlice[s];
+            const long long base = (long long)S.start64 * SLICE_ROWS;
+            for (int q = 0; q < SLICE_ROWS; q++) {
+                const int r = s * SLICE_ROWS + q, c = iperm[r];
+                int j = 0;
+                if (c >= 0) {
+                    for (int f = ownerStart[c]; f < ownerStart[c + 1]; f++, j++) {
+                        const int n = perm[u[f]];
+                        const uint32_t t = (n >= r0 && n < r1) ? slotOf(n, 1 + nbSlot[f]) : FS_NONE;
+                        fsCT[base + (long long)j * SLICE_ROWS + q] = colOf(n) | t << 16;
+                        fsCode[base + (long long)j * SLICE_ROWS + q] = 2 * f;
+                    }
+                }
+                for (; j < S.wo; j++) {
+                    fsCT[base + (long long)j * SLICE_ROWS + q] = (uint32_t)(r - r0) | FS_PAD << 16;
+                    fsCode[base + (long long)j * SLICE_ROWS + q] = -1;
+                }
+            }
+        }
+        int ix = fsListStart[b], ii = fsListIfc[b];
+        for (int r = r0; r < r1; r++) {
+            const int c = iperm[r];
+            if (c < 0) continue;
+            for (int k = losortStart[c]; k < losortStart[c + 1]; k++) {
+                const int f = losort[k], o = perm[l[f]];
+                if (o >= r0 && o < r1) continue;
+                fsCT[ix] = colOf(o) | slotOf(r, 1 + (k - losortStart[c])) << 16;
+                fsCode[ix++] = 2 * f + 1;
+            }
+            const int wn = fsSlice[r / SLICE_ROWS].wn;
+            for (int k = pfStart[c]; k < pfStart[c + 1]; k++) {
+                fsCT[ii] = colOf(nPad + pfItem[k]) | slotOf(r, 1 + wn + (k - pfStart[c])) << 16;
+                fsCode[ii++] = -2 - pfItem[k];
+            }
+        }
     }
     if (tooWide) {
         if (bandRows > SLICE_ROWS) { // retry with narrower bands (see the tile check below)
@@ -405,6 +521,21 @@ int layout_build(b200ldu_addr *a, const double *centres)
     std::vector<int> sendRows(std::max(nRecv, 1));
     for (int i = 0; i < nRecv; i++) sendRows[i] = perm[a->faceCells[i]];
 
+    // The face stream's CTAs hold the product buffer next to the tile.  It is used where that still leaves as many
+    // CTAs per SM as the entry stream's tile alone (large meshes with 512-row bands; not the one-wave bands of mid-size
+    // meshes nor GAMG levels with many faces per row).  B200LDU_FACE_STREAM=0 never uses it, =1 whenever it fits.
+    {
+        const long long tile = ((long long)bandRows + maxHalo + 1) & ~1ll;
+        const bool fitsSmem = (size_t)(tile + fsBufMax) * sizeof(double) <= TILE_BYTES_MAX;
+        a->hasFs = fsFits && fitsSmem && ctas_per_sm(tile + fsBufMax) >= ctas_per_sm(tile);
+        if (const char *e = getenv("B200LDU_FACE_STREAM")) {
+            if (!strcmp(e, "0")) a->hasFs = false;
+            if (!strcmp(e, "1")) a->hasFs = fsFits && fitsSmem;
+        }
+        a->fsOwn = fsOwn;
+        a->fsList = fsList;
+    }
+
     a->nEntries = nEntries;
     a->nHaloTotal = haloStart[nBands];
     a->vecLen = ((long long)nPad + nRecv + 1) & ~1ll;
@@ -423,6 +554,14 @@ int layout_build(b200ldu_addr *a, const double *centres)
         a->dbg_code.swap(code);
         a->dbg_haloStart.swap(haloStart);
         a->dbg_haloIdx.swap(haloIdx);
+        if (fsFits) { // built whether or not the engine would use it, so that its structure can be checked
+            a->dbg_fsSlice.swap(fsSlice);
+            a->dbg_fsCT.swap(fsCT);
+            a->dbg_fsCode.swap(fsCode);
+            a->dbg_fsListStart.swap(fsListStart);
+            a->dbg_fsListIfc.swap(fsListIfc);
+        }
+        a->L.fsBufMax = (int)fsBufMax;
         return B200LDU_OK;
     }
 
@@ -442,8 +581,20 @@ int layout_build(b200ldu_addr *a, const double *centres)
     TRY(dev_upload(&a->d_ownerStart, ownerStart));
     TRY(dev_upload(&a->d_losort, losort));
     TRY(dev_upload(&a->d_losortStart, losortStart));
+    if (a->hasFs) {
+        TRY(dev_upload(&a->d_fsSlice, fsSlice));
+        TRY(dev_upload(&a->d_fsCT, fsCT));
+        TRY(dev_upload(&a->d_fsCode, fsCode));
+        TRY(dev_upload(&a->d_fsListStart, fsListStart));
+        TRY(dev_upload(&a->d_fsListIfc, fsListIfc));
+    }
 
     LayoutDev &L = a->L;
+    L.fsSlice = a->d_fsSlice;
+    L.fsCT = a->d_fsCT;
+    L.fsListStart = a->d_fsListStart;
+    L.fsListIfc = a->d_fsListIfc;
+    L.fsBufMax = a->hasFs ? (int)fsBufMax : 0;
     L.nCells = nCells;
     L.nPad = nPad;
     L.nBands = nBands;
@@ -496,6 +647,9 @@ extern "C" int b200ldu_layout_debug_create(int nCells, int nFaces, const int *lo
 
 // what: 0 perm(int32) 1 iperm(int32) 2 sliceStart(int64) 3 sliceW(u16) 4 sliceWL(u16) 5 col(u16)
 //       6 code(int32) 7 haloStart(int32) 8 haloIdx(int32) 9 dims {nPad,nBands,bandRows,nRecv,maxHalo}(int32)
+//       face stream (empty when it was not built): 10 fsSlice (4 int32 per slice: start64, bufOff, wo | wn << 16,
+//       wi) 11 fsCT(u32) 12 fsCode(int32) 13 fsListStart(int32) 14 fsListIfc(int32)
+//       15 fs dims {fsOwn, fsList, fsBufMax, hasFs}(int64)
 // returns the element count (copies min(count, cap) elements when out != NULL)
 extern "C" long long b200ldu_layout_debug_get(const b200ldu_addr *a, int what, void *out, long long cap)
 {
@@ -516,6 +670,15 @@ extern "C" long long b200ldu_layout_debug_get(const b200ldu_addr *a, int what, v
     case 7: return give(a->dbg_haloStart.data(), 4, (long long)a->dbg_haloStart.size());
     case 8: return give(a->dbg_haloIdx.data(), 4, a->nHaloTotal);
     case 9: return give(dims, 4, 5);
+    case 10: return give(a->dbg_fsSlice.data(), 4, 4 * (long long)a->dbg_fsSlice.size());
+    case 11: return give(a->dbg_fsCT.data(), 4, a->dbg_fsCT.empty() ? 0 : a->fsOwn + a->fsList);
+    case 12: return give(a->dbg_fsCode.data(), 4, a->dbg_fsCode.empty() ? 0 : a->fsOwn + a->fsList);
+    case 13: return give(a->dbg_fsListStart.data(), 4, (long long)a->dbg_fsListStart.size());
+    case 14: return give(a->dbg_fsListIfc.data(), 4, (long long)a->dbg_fsListIfc.size());
+    case 15: {
+        long long fd[4] = {a->fsOwn, a->fsList, a->L.fsBufMax, a->hasFs ? 1 : 0};
+        return give(fd, 8, 4);
+    }
     }
     return -1;
 }

@@ -204,7 +204,8 @@ extern "C" int b200ldu_addr_destroy(b200ldu_addr *a)
                     a->d_ownerStart, a->d_losort, a->d_losortStart, a->d_bFaceCells, a->d_cyclicSrc,
                     a->d_bCellStart, a->d_bCellFaces, a->d_bCells, a->d_packPatches, a->d_packChunks,
                     a->d_cCellStart, a->d_cCellFaces, a->d_cFaceCells, a->d_mulesScratch, a->d_fvmScratch[0],
-                    a->d_fvmScratch[1], a->d_fvmScratch[2], a->d_fvmScratch[3]};
+                    a->d_fvmScratch[1], a->d_fvmScratch[2], a->d_fvmScratch[3], a->d_fsSlice, a->d_fsCT, a->d_fsCode,
+                    a->d_fsListStart, a->d_fsListIfc};
     for (void *p : ptrs)
         if (p) cudaFree(p);
     for (double *p : a->pool)
@@ -222,6 +223,17 @@ extern "C" int b200ldu_addr_info(const b200ldu_addr *a, long long *nPadRows, lon
     if (nHalo) *nHalo = a->nHaloTotal;
     if (bandRows) *bandRows = a->L.bandRows;
     if (nBands) *nBands = a->L.nBands;
+    return B200LDU_OK;
+}
+
+extern "C" int b200ldu_addr_face_info(const b200ldu_addr *a, long long *nOwnerSlots, long long *nListItems,
+                                      int *bufDoubles, int *used)
+{
+    if (!a) return B200LDU_EINVAL;
+    if (nOwnerSlots) *nOwnerSlots = a->fsOwn;
+    if (nListItems) *nListItems = a->fsList;
+    if (bufDoubles) *bufDoubles = a->L.fsBufMax;
+    if (used) *used = a->hasFs ? 1 : 0;
     return B200LDU_OK;
 }
 
@@ -324,7 +336,7 @@ extern "C" int b200ldu_matrix_destroy(b200ldu_matrix *m)
     cudaSetDevice(m->a->ctx->device);
     cudaStreamSynchronize(m->a->ctx->stream);
     if (m->d_valT && m->d_valT != m->d_val) cudaFree(m->d_valT);
-    void *ptrs[] = {m->d_val, m->d_diag, m->d_rD, m->d_partials, m->d_scal, m->d_hist, m->d_sendBuf,
+    void *ptrs[] = {m->d_val, m->d_fval, m->d_diag, m->d_rD, m->d_partials, m->d_scal, m->d_hist, m->d_sendBuf,
                     m->own[0], m->own[1], m->own[2], m->own[3], m->own[4]};
     for (void *p : ptrs)
         if (p) cudaFree(p);
@@ -437,6 +449,27 @@ extern "C" int b200ldu_matrix_set(b200ldu_matrix *m, const double *diag_d, const
     // Tmul needs its own coefficient stream when A != A^T (asymmetric coefficients or
     // interfaceIntCoeffs != interfaceBouCoeffs)
     bool needT = !m->symmetric || (a->L.nRecv && !sameIfc);
+    if (!needT && a->hasFs) {
+        // A == A^T: the face stream holds every face once and serves both
+        if (m->d_valT && m->d_valT != m->d_val) cudaFree(m->d_valT);
+        if (m->d_val) cudaFree(m->d_val);
+        m->d_val = m->d_valT = nullptr;
+        const long long nf = a->fsOwn + a->fsList;
+        if (!m->d_fval) CUDA_TRY(cudaMalloc((void **)&m->d_fval, sizeof(double) * (size_t)(nf > 0 ? nf : 1)));
+        if (nf > 0) {
+            fill_val_kernel<<<(unsigned)((nf + 255) / 256), 256, 0, st>>>(nf, a->d_fsCode, up, lo, bo, m->d_fval, 0);
+            a->ctx->launches++;
+        }
+        KERNEL_CHECK();
+        m->haveT = false;
+        m->upper_ext = up;
+        m->bou_ext = bo;
+        m->int_ext = in;
+        m->lower_ext = lo;
+        return matrix_set_diag(m, dg);
+    }
+    if (m->d_fval) cudaFree(m->d_fval);
+    m->d_fval = nullptr;
     size_t nb = sizeof(double) * (size_t)(ne > 0 ? ne : 1);
     if (!m->d_val) CUDA_TRY(cudaMalloc((void **)&m->d_val, nb));
     if (needT && (!m->d_valT || m->d_valT == m->d_val)) {

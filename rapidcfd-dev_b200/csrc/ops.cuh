@@ -28,11 +28,10 @@ struct OpBase {
     int waitHalo = 0; // 1: a peer-memory halo exchange of the staged vector is in flight
     // first thing every CTA of an engine kernel does; false => the CTA exits (the device has decided to stop)
     __device__ __forceinline__ bool prologue(const LayoutDev &) const { return !(stop && *stop); }
-    // row-sum term acc + v*a; Residual, OffDiag and CoeffSum replace it
-    __device__ __forceinline__ double term(double acc, double v, double a) const
-    {
-        return __dadd_rn(acc, __dmul_rn(v, a));
-    }
+    // row-sum terms: add(acc, prod(v, a)) = acc + v*a; Residual, OffDiag and CoeffSum replace them
+    __device__ __forceinline__ double prod(double v, double a) const { return __dmul_rn(v, a); }
+    __device__ __forceinline__ double add(double acc, double p) const { return __dadd_rn(acc, p); }
+    __device__ __forceinline__ double identity() const { return -0.0; } // x + -0 == x, also for x = -0
 };
 
 // operators that stage the vector x unchanged
@@ -141,10 +140,8 @@ struct ResidualOp : StageXOp {
     const double *diag, *b;
     double *out;
     __device__ __forceinline__ double init(int r, double a) const { return __dsub_rn(b[r], __dmul_rn(diag[r], a)); }
-    __device__ __forceinline__ double term(double acc, double v, double a) const
-    {
-        return __dsub_rn(acc, __dmul_rn(v, a));
-    }
+    __device__ __forceinline__ double add(double acc, double p) const { return __dsub_rn(acc, p); }
+    __device__ __forceinline__ double identity() const { return 0.0; } // x - +0 == x
     __device__ __forceinline__ void finish(int r, double acc0, double acc1, double, double, double *red) const
     {
         *reinterpret_cast<double2 *>(out + r) = make_double2(acc0, acc1);
@@ -162,10 +159,9 @@ struct CoeffSumOp : OpBase {
     __device__ __forceinline__ double stage(int) const { return 0.0; }
     __device__ __forceinline__ double2 stage_own(int) const { return make_double2(0, 0); }
     __device__ __forceinline__ double init(int r, double) const { return diag ? diag[r] : 0.0; }
-    __device__ __forceinline__ double term(double acc, double v, double) const
-    {
-        return NEG_ ? __dsub_rn(acc, v) : __dadd_rn(acc, v);
-    }
+    __device__ __forceinline__ double prod(double v, double) const { return v; }
+    __device__ __forceinline__ double add(double acc, double p) const { return NEG_ ? __dsub_rn(acc, p) : __dadd_rn(acc, p); }
+    __device__ __forceinline__ double identity() const { return NEG_ ? 0.0 : -0.0; }
     __device__ __forceinline__ void finish(int r, double acc0, double acc1, double, double, double *) const
     {
         *reinterpret_cast<double2 *>(out + r) = make_double2(acc0, acc1);
@@ -181,10 +177,8 @@ struct OffDiagOp : StageXOp {
     const double *diag;
     double *out;
     __device__ __forceinline__ double init(int, double) const { return 0.0; }
-    __device__ __forceinline__ double term(double acc, double v, double a) const
-    {
-        return DIVDIAG_ ? OpBase::term(acc, v, a) : __dsub_rn(acc, __dmul_rn(v, a));
-    }
+    __device__ __forceinline__ double add(double acc, double p) const { return DIVDIAG_ ? __dadd_rn(acc, p) : __dsub_rn(acc, p); }
+    __device__ __forceinline__ double identity() const { return DIVDIAG_ ? -0.0 : 0.0; }
     __device__ __forceinline__ void finish(int r, double acc0, double acc1, double, double, double *) const
     {
         if (DIVDIAG_) {
