@@ -268,7 +268,6 @@ int comm_addr_setup(b200ldu_addr *a)
     a->L.tail1 = a->L.tail0 + P2P_RECV_CAP;
     a->L.packChunks = d_pc;
     a->L.packPatches = d_pp;
-    a->L.sendRows = a->d_sendRows;
     a->L.seqs = ctx->d_seq;
     a->L.nPackChunks = (int)pc.size();
     a->p2pHalo = true;
@@ -314,7 +313,7 @@ int comm_halo_exchange(b200ldu_addr *a, double *x, double *sendBuf, const int *s
         KERNEL_CHECK();
     }
     if (!remote) return B200LDU_OK;
-    pack_kernel<<<(nRecv + 255) / 256, 256, 0, ctx->stream>>>(nRecv, a->d_sendRows, x, sendBuf, stop);
+    pack_kernel<<<(nRecv + 255) / 256, 256, 0, ctx->stream>>>(nRecv, a->L.sendRows, x, sendBuf, stop);
     ctx->launches++;
     KERNEL_CHECK();
     if (remote && !ctx->nccl) {

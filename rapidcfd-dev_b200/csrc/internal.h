@@ -144,6 +144,28 @@ struct LayoutDev {
     int nPackChunks;
 };
 
+// Host arrays of the banded layout, as layout_build produces them: a device addressing uploads them (into L), the
+// host-only structural self-check keeps them (b200ldu_layout_debug_get).
+struct LayoutHost {
+    int nPad = 0, nBands = 0, bandRows = 0, nRecv = 0, maxHalo = 0;
+    long long nEntries = 0;
+    // face stream: stored owner slots (padding included), list items, product-buffer doubles of the largest band,
+    // and whether symmetric matrices use it
+    long long fsOwn = 0, fsList = 0, fsBufMax = 0;
+    bool hasFs = false;
+    // entry stream
+    std::vector<long long> sliceStart;
+    std::vector<uint16_t> sliceW, sliceWL, col;
+    std::vector<int> code;
+    // halo
+    std::vector<int> haloStart, haloIdx;
+    std::vector<int> sendRows; // [nRecv] banded row of faceCells
+    // face stream (empty where it was not built)
+    std::vector<FsSlice> fsSlice;
+    std::vector<uint32_t> fsCT;
+    std::vector<int> fsCode, fsListStart, fsListIfc;
+};
+
 struct b200ldu_addr {
     b200ldu_ctx *ctx = nullptr;
     int nCells = 0, nFaces = 0;
@@ -156,19 +178,14 @@ struct b200ldu_addr {
     long long nHaloTotal = 0;
     std::vector<int> perm_h, iperm_h;
     std::vector<double> centres_h; // optional cell centres (kept for GAMG coarse-level banding)
-    // device arrays owned
-    long long *d_sliceStart = nullptr;
-    uint16_t *d_sliceW = nullptr, *d_sliceWL = nullptr, *d_col = nullptr;
+    // device arrays owned: layoutMem holds every array layout_build uploaded (L's arrays, d_code, d_fsCode and the
+    // caller-order CSR views d_l .. d_losortStart); the other pointers below own their arrays
+    std::vector<void *> layoutMem;
     int *d_code = nullptr; // [nEntries] value source: 2f+side | -1 pad | -2-pf interface
     // face stream: used by symmetric matrices when the layout has one (hasFs)
     bool hasFs = false;
     long long fsOwn = 0, fsList = 0; // stored owner slots (padding included), list items
-    FsSlice *d_fsSlice = nullptr;
-    uint32_t *d_fsCT = nullptr;
     int *d_fsCode = nullptr; // [fsOwn + fsList] value source, as d_code
-    int *d_fsListStart = nullptr, *d_fsListIfc = nullptr;
-    int *d_haloStart = nullptr, *d_haloIdx = nullptr, *d_perm = nullptr, *d_iperm = nullptr;
-    int *d_sendRows = nullptr; // [nRecv] banded row of faceCells (pack kernel)
     bool p2pHalo = false;      // peer-store halo usable for this addressing
     void *d_packPatches = nullptr, *d_packChunks = nullptr; // PackPatch[], PackChunk[] (comm.cu)
     int nPackChunks = 0;
@@ -191,12 +208,7 @@ struct b200ldu_addr {
     size_t fvmScratchLen[4] = {0, 0, 0, 0};
     // host-only structural self-check (b200ldu_layout_debug_*): no GPU, no compute
     bool hostOnly = false;
-    std::vector<long long> dbg_sliceStart;
-    std::vector<uint16_t> dbg_sliceW, dbg_sliceWL, dbg_col;
-    std::vector<int> dbg_code, dbg_haloStart, dbg_haloIdx;
-    std::vector<FsSlice> dbg_fsSlice;
-    std::vector<uint32_t> dbg_fsCT;
-    std::vector<int> dbg_fsCode, dbg_fsListStart, dbg_fsListIfc;
+    LayoutHost host;
     // workspace pool for caller-order entry points (banded vectors)
     std::vector<double *> pool;
     long long vecLen = 0; // nPad + nRecv (padded to even)

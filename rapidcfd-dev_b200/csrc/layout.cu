@@ -15,6 +15,10 @@
 //  * columns are 16-bit indices into the band's shared-memory psi tile: the band's own
 //    rows first, then the band's halo list (rows of other bands / received interface
 //    values) which is gathered once per band.
+//
+// layout_build runs in stages: addressing checks and CSR, renumbering, coupled-patch face
+// lists, then a plan for a band size (halved until the band fits), the face-stream choice,
+// and the fills of the entry stream and (where it is used) the face stream.
 #include <algorithm>
 #include <cmath>
 #include <cstdlib>
@@ -25,8 +29,12 @@
 
 namespace {
 
-struct Csr {
-    std::vector<int> start, item;
+// the addressing seen from both sides of every face, and each cell's coupled-patch faces
+struct Graph {
+    int nCells, nFaces, nRecv;
+    const std::vector<int> &l, &u;
+    std::vector<int> ownerStart, losortStart, losort;
+    std::vector<int> pfStart, pfItem; // cell -> coupled-patch faces, in (patch, patch face) order
 };
 
 // cell -> faces it owns is contiguous (faces sorted by owner); cell -> faces where it
@@ -52,26 +60,24 @@ void build_owner_start(int nCells, const std::vector<int> &l, std::vector<int> &
 
 // breadth-first graph distance from `seed` (used when no cell centres are given);
 // further components, if any, restart from their lowest cell
-void bfs_dist(int nCells, const std::vector<int> &l, const std::vector<int> &u,
-              const std::vector<int> &ownerStart, const std::vector<int> &losortStart,
-              const std::vector<int> &losort, int seed, std::vector<int> &dist)
+void bfs_dist(const Graph &g, int seed, std::vector<int> &dist)
 {
-    dist.assign(nCells, -1);
+    dist.assign(g.nCells, -1);
     std::vector<int> q;
-    q.reserve(nCells);
+    q.reserve(g.nCells);
     auto grow = [&](int s) {
         size_t head = q.size();
         dist[s] = 0;
         q.push_back(s);
         while (head < q.size()) {
             int c = q[head++];
-            for (int f = ownerStart[c]; f < ownerStart[c + 1]; f++)
-                if (dist[u[f]] < 0) {
-                    dist[u[f]] = dist[c] + 1;
-                    q.push_back(u[f]);
+            for (int f = g.ownerStart[c]; f < g.ownerStart[c + 1]; f++)
+                if (dist[g.u[f]] < 0) {
+                    dist[g.u[f]] = dist[c] + 1;
+                    q.push_back(g.u[f]);
                 }
-            for (int k = losortStart[c]; k < losortStart[c + 1]; k++) {
-                int nb = l[losort[k]];
+            for (int k = g.losortStart[c]; k < g.losortStart[c + 1]; k++) {
+                int nb = g.l[g.losort[k]];
                 if (dist[nb] < 0) {
                     dist[nb] = dist[c] + 1;
                     q.push_back(nb);
@@ -80,7 +86,7 @@ void bfs_dist(int nCells, const std::vector<int> &l, const std::vector<int> &u,
         }
     };
     grow(seed);
-    for (int c = 0; c < nCells; c++)
+    for (int c = 0; c < g.nCells; c++)
         if (dist[c] < 0) grow(c);
 }
 
@@ -102,16 +108,12 @@ uint64_t interleave(const uint32_t idx[3], const int bits[3])
     return code;
 }
 
-// set while layout_build retries with narrower bands (tile did not fit in shared memory)
-thread_local int g_bandRowsRetry = 0;
-
-// a band's tile is (bandRows + halo) doubles per staged vector, two vectors at most (engine.cuh);
-// H100 gives a CTA up to 227 KB, the kernel keeps a little static scratch
+// a band's tile is (bandRows + halo) doubles of the one staged vector (engine.cuh); H100 gives a CTA up to 227 KB,
+// the kernel keeps a little static scratch
 constexpr size_t TILE_BYTES_MAX = 200 * 1024;
 
 int pick_band_rows(int nCells, int smCount, int packCtas)
 {
-    if (g_bandRowsRetry) return g_bandRowsRetry;
     if (const char *e = getenv("B200LDU_BAND_ROWS")) {
         int v = atoi(e);
         if (v >= SLICE_ROWS && v % SLICE_ROWS == 0 && v <= 16384) return v;
@@ -155,50 +157,41 @@ int ctas_per_sm(long long smemDoubles)
     return (int)std::min<long long>(6, 228 * 1024 / per);
 }
 
-} // namespace
-
-int layout_build(b200ldu_addr *a, const double *centres)
+// ---- 1. addressing checks and CSR --------------------------------------------
+int build_csr(Graph &g)
 {
-    const int nCells = a->nCells, nFaces = a->nFaces;
-    const std::vector<int> &l = a->l, &u = a->u;
-    if (nCells <= 0) {
+    if (g.nCells <= 0) {
         b200_set_error("layout_build: nCells must be positive");
         return B200LDU_EINVAL;
     }
-    for (int f = 0; f < nFaces; f++) {
-        if (l[f] < 0 || u[f] >= nCells || l[f] >= u[f] || (f && l[f] < l[f - 1])) {
+    for (int f = 0; f < g.nFaces; f++) {
+        if (g.l[f] < 0 || g.u[f] >= g.nCells || g.l[f] >= g.u[f] || (f && g.l[f] < g.l[f - 1])) {
             b200_set_error("layout_build: face %d violates upper-triangular owner-sorted order", f);
             return B200LDU_EINVAL;
         }
     }
-    std::vector<int> ownerStart, losortStart, losort;
-    build_owner_start(nCells, l, ownerStart);
-    build_losort(nCells, u, losortStart, losort);
+    build_owner_start(g.nCells, g.l, g.ownerStart);
+    build_losort(g.nCells, g.u, g.losortStart, g.losort);
+    return B200LDU_OK;
+}
 
-    int packCtas = 0;
-    for (int p = 0; p < a->nPatches; p++)
-        if (p < (int)a->neighbRank.size() && a->neighbRank[p] >= 0) packCtas += (a->patchStart[p + 1] - a->patchStart[p] + PACK_CHUNK - 1) / PACK_CHUNK;
-    const int bandRows = pick_band_rows(nCells, a->ctx ? a->ctx->smCount : 132, packCtas);
-    const int nBands = (nCells + bandRows - 1) / bandRows;
-    const int nPad = nBands * bandRows;
-    const int slicesPerBand = bandRows / SLICE_ROWS;
-    const int nSlices = nPad / SLICE_ROWS;
-    const int nRecv = a->nPatches ? a->patchStart[a->nPatches] : 0;
-
-    // ---- 1. cell renumbering ------------------------------------------------
+// ---- 2. cell renumbering: banded row -> caller cell, whatever the band size ----
+std::vector<int> renumber(const Graph &g, const double *centres)
+{
+    const int nCells = g.nCells;
     std::vector<double> emb; // 3 coordinates per cell
     const double *xyz = centres;
     if (!xyz) {
         std::vector<int> d0, d1, d2, d3;
-        bfs_dist(nCells, l, u, ownerStart, losortStart, losort, 0, d0);
+        bfs_dist(g, 0, d0);
         int s1 = argmax(d0);
-        bfs_dist(nCells, l, u, ownerStart, losortStart, losort, s1, d1);
+        bfs_dist(g, s1, d1);
         int s2 = argmax(d1);
-        bfs_dist(nCells, l, u, ownerStart, losortStart, losort, s2, d2);
+        bfs_dist(g, s2, d2);
         std::vector<int> sum(nCells);
         for (int c = 0; c < nCells; c++) sum[c] = d1[c] + d2[c];
         int s3 = argmax(sum);
-        bfs_dist(nCells, l, u, ownerStart, losortStart, losort, s3, d3);
+        bfs_dist(g, s3, d3);
         emb.resize((size_t)3 * nCells);
         for (int c = 0; c < nCells; c++) {
             emb[3 * (size_t)c + 0] = d1[c];
@@ -247,98 +240,108 @@ int layout_build(b200ldu_addr *a, const double *centres)
         }
         key[c] = interleave(idx, bits);
     }
-    std::vector<int> order(nCells); // banded row -> caller cell
-    {
-        int kb = bits[0] + bits[1] + bits[2];
-        if (kb <= 26) { // counting sort (stable => caller order inside a tile)
-            size_t nT = (size_t)1 << kb;
-            std::vector<int> cnt(nT + 1, 0);
-            for (int c = 0; c < nCells; c++) cnt[key[c] + 1]++;
-            for (size_t t = 0; t < nT; t++) cnt[t + 1] += cnt[t];
-            for (int c = 0; c < nCells; c++) order[cnt[key[c]]++] = c;
-        } else {
-            std::iota(order.begin(), order.end(), 0);
-            std::stable_sort(order.begin(), order.end(),
-                             [&](int x, int y) { return key[x] < key[y]; });
-        }
+    std::vector<int> order(nCells);
+    int kb = bits[0] + bits[1] + bits[2];
+    if (kb <= 26) { // counting sort (stable => caller order inside a tile)
+        size_t nT = (size_t)1 << kb;
+        std::vector<int> cnt(nT + 1, 0);
+        for (int c = 0; c < nCells; c++) cnt[key[c] + 1]++;
+        for (size_t t = 0; t < nT; t++) cnt[t + 1] += cnt[t];
+        for (int c = 0; c < nCells; c++) order[cnt[key[c]]++] = c;
+    } else {
+        std::iota(order.begin(), order.end(), 0);
+        std::stable_sort(order.begin(), order.end(), [&](int x, int y) { return key[x] < key[y]; });
     }
-    key.clear();
-    key.shrink_to_fit();
-    a->perm_h.assign(nCells, 0);
-    a->iperm_h.assign(nPad, -1);
-    for (int r = 0; r < nCells; r++) {
-        a->perm_h[order[r]] = r;
-        a->iperm_h[r] = order[r];
-    }
-    const std::vector<int> &perm = a->perm_h, &iperm = a->iperm_h;
+    return order;
+}
 
-    // cell -> coupled-patch faces, in (patch, patch face) order
-    std::vector<int> pfStart((size_t)nCells + 1, 0), pfItem(nRecv);
-    for (int i = 0; i < nRecv; i++) pfStart[a->faceCells[i] + 1]++;
-    for (int c = 0; c < nCells; c++) pfStart[c + 1] += pfStart[c];
-    {
-        std::vector<int> cur(pfStart.begin(), pfStart.end() - 1);
-        for (int i = 0; i < nRecv; i++) pfItem[cur[a->faceCells[i]]++] = i;
-    }
+// ---- 3. cell -> coupled-patch faces -------------------------------------------
+void build_patch_faces(const std::vector<int> &faceCells, Graph &g)
+{
+    g.pfStart.assign((size_t)g.nCells + 1, 0);
+    g.pfItem.resize(g.nRecv);
+    for (int i = 0; i < g.nRecv; i++) g.pfStart[faceCells[i] + 1]++;
+    for (int c = 0; c < g.nCells; c++) g.pfStart[c + 1] += g.pfStart[c];
+    std::vector<int> cur(g.pfStart.begin(), g.pfStart.end() - 1);
+    for (int i = 0; i < g.nRecv; i++) g.pfItem[cur[faceCells[i]]++] = i;
+}
 
-    // ---- 2. slice widths ----------------------------------------------------
-    std::vector<uint16_t> sliceW(nSlices, 0), sliceWL(nSlices, 0);
+// ---- 4. plan for one band size --------------------------------------------------
+// Everything but the two streams' entries: slice widths and offsets of both streams, the face stream's list bounds,
+// the per-band halo lists and whether the band fits.
+struct Plan {
+    LayoutHost H;
+    std::vector<int> iperm;             // [nPad] banded row -> caller cell, -1 padding
+    std::vector<std::vector<int>> halo; // per band: extended indices of its outside columns, sorted
+    int tooWide = 0;                    // bands with more than 65535 tile columns
+    bool tileFits = false;              // the tile of every band fits in shared memory
+    bool fsFits = false;                // the 16-bit product slots address the buffer, the 32-bit offsets every entry
+};
+
+int plan_layout(const Graph &g, const std::vector<int> &order, const std::vector<int> &perm, int bandRows, Plan &P)
+{
+    P = Plan{};
+    LayoutHost &H = P.H;
+    const int nBands = (g.nCells + bandRows - 1) / bandRows;
+    const int nPad = nBands * bandRows;
+    const int slicesPerBand = bandRows / SLICE_ROWS;
+    const int nSlices = nPad / SLICE_ROWS;
+    H.nPad = nPad;
+    H.nBands = nBands;
+    H.bandRows = bandRows;
+    H.nRecv = g.nRecv;
+    P.iperm = order;
+    P.iperm.resize(nPad, -1);
+    const std::vector<int> &iperm = P.iperm;
+
+    // slice widths: entry stream (owner + neighbour entries, then interfaces) and face stream (owner entries; buffer
+    // slots for neighbour and interface products)
+    H.sliceW.assign(nSlices, 0);
+    H.sliceWL.assign(nSlices, 0);
+    H.fsSlice.assign(nSlices, FsSlice{});
     int bad = 0;
 #pragma omp parallel for schedule(static) reduction(+ : bad)
     for (int s = 0; s < nSlices; s++) {
-        int wl = 0, wi = 0;
+        int wl = 0, wo = 0, wn = 0, wi = 0;
         for (int q = 0; q < SLICE_ROWS; q++) {
             int c = iperm[(size_t)s * SLICE_ROWS + q];
             if (c < 0) continue;
-            int nl = (ownerStart[c + 1] - ownerStart[c]) + (losortStart[c + 1] - losortStart[c]);
-            int ni = pfStart[c + 1] - pfStart[c];
-            wl = std::max(wl, nl);
-            wi = std::max(wi, ni);
+            const int no = g.ownerStart[c + 1] - g.ownerStart[c], nn = g.losortStart[c + 1] - g.losortStart[c];
+            wl = std::max(wl, no + nn);
+            wo = std::max(wo, no);
+            wn = std::max(wn, nn);
+            wi = std::max(wi, g.pfStart[c + 1] - g.pfStart[c]);
         }
         if (wl + wi > 65535) bad++;
-        sliceWL[s] = (uint16_t)wl;
-        sliceW[s] = (uint16_t)(wl + wi);
+        H.sliceWL[s] = (uint16_t)wl;
+        H.sliceW[s] = (uint16_t)(wl + wi);
+        H.fsSlice[s] = FsSlice{0, 0, (uint16_t)wo, (uint16_t)wn, (uint16_t)wi, 0};
     }
     if (bad) {
         b200_set_error("layout_build: a row has more than 65535 entries");
         return B200LDU_ELAYOUT;
     }
-    std::vector<long long> sliceStart((size_t)nSlices + 1, 0);
+    H.sliceStart.assign((size_t)nSlices + 1, 0);
     for (int s = 0; s < nSlices; s++)
-        sliceStart[s + 1] = sliceStart[s] + (long long)sliceW[s] * SLICE_ROWS;
-    const long long nEntries = sliceStart[nSlices];
+        H.sliceStart[s + 1] = H.sliceStart[s] + (long long)H.sliceW[s] * SLICE_ROWS;
+    H.nEntries = H.sliceStart[nSlices];
 
-    // ---- 2b. face stream: slice widths, product-buffer offsets, list sizes ----
-    // nbSlot[f]: position of face f among its neighbour cell's losort faces
-    std::vector<int> nbSlot((size_t)std::max(nFaces, 1));
-    for (int c = 0; c < nCells; c++)
-        for (int k = losortStart[c]; k < losortStart[c + 1]; k++) nbSlot[losort[k]] = k - losortStart[c];
-    std::vector<FsSlice> fsSlice(nSlices);
-#pragma omp parallel for schedule(static)
-    for (int s = 0; s < nSlices; s++) {
-        int wo = 0, wn = 0, wi = 0;
-        for (int q = 0; q < SLICE_ROWS; q++) {
-            int c = iperm[(size_t)s * SLICE_ROWS + q];
-            if (c < 0) continue;
-            wo = std::max(wo, ownerStart[c + 1] - ownerStart[c]);
-            wn = std::max(wn, losortStart[c + 1] - losortStart[c]);
-            wi = std::max(wi, pfStart[c + 1] - pfStart[c]);
-        }
-        fsSlice[s] = FsSlice{0, 0, (uint16_t)wo, (uint16_t)wn, (uint16_t)wi, 0};
-    }
-    long long fsBufMax = 0, fsOwn = 0;
+    // face stream: owner-stream and product-buffer offsets of each slice, then the list bounds of each band
+    long long fsOwn = 0;
     for (int b = 0; b < nBands; b++) {
         long long off = 0;
         for (int sl = 0; sl < slicesPerBand; sl++) {
-            FsSlice &S = fsSlice[(size_t)b * slicesPerBand + sl];
+            FsSlice &S = H.fsSlice[(size_t)b * slicesPerBand + sl];
             S.start64 = (int)(fsOwn / SLICE_ROWS);
             S.bufOff = (int)std::min<long long>(off, INT32_MAX);
             fsOwn += (long long)S.wo * SLICE_ROWS;
             off += (1 + (long long)S.wn + S.wi) * SLICE_ROWS;
         }
-        fsBufMax = std::max(fsBufMax, off);
+        H.fsBufMax = std::max(H.fsBufMax, off);
     }
-    std::vector<int> fsListStart((size_t)nBands + 1, 0), fsListIfc(nBands, 0); // counts first
+    std::vector<int> &fsListStart = H.fsListStart, &fsListIfc = H.fsListIfc;
+    fsListStart.assign((size_t)nBands + 1, 0); // counts first
+    fsListIfc.assign(nBands, 0);
 #pragma omp parallel for schedule(static)
     for (int b = 0; b < nBands; b++) {
         const int r0 = b * bandRows, r1 = r0 + bandRows;
@@ -346,11 +349,11 @@ int layout_build(b200ldu_addr *a, const double *centres)
         for (int r = r0; r < r1; r++) {
             int c = iperm[r];
             if (c < 0) continue;
-            for (int k = losortStart[c]; k < losortStart[c + 1]; k++) {
-                int t = perm[l[losort[k]]];
+            for (int k = g.losortStart[c]; k < g.losortStart[c + 1]; k++) {
+                int t = perm[g.l[g.losort[k]]];
                 nx += (t < r0 || t >= r1);
             }
-            ni += pfStart[c + 1] - pfStart[c];
+            ni += g.pfStart[c + 1] - g.pfStart[c];
         }
         fsListIfc[b] = nx;
         fsListStart[b + 1] = nx + ni;
@@ -361,62 +364,101 @@ int layout_build(b200ldu_addr *a, const double *centres)
         fsListIfc[b] += fsListStart[b];
         fsListStart[b + 1] = (int)std::min<long long>(next, INT32_MAX);
     }
-    const long long fsList = (long long)fsListStart[nBands] - fsListStart[0];
-    // the 16-bit product slots must address the whole buffer, the 32-bit stream offsets every entry
-    bool fsFits = fsBufMax < (long long)FS_PAD && fsOwn + fsList < INT32_MAX;
-    std::vector<uint32_t> fsCT(fsFits ? (size_t)std::max<long long>(fsOwn + fsList, 1) : 1);
-    std::vector<int> fsCode(fsCT.size());
+    H.fsOwn = fsOwn;
+    H.fsList = (long long)fsListStart[nBands] - fsListStart[0];
+    P.fsFits = H.fsBufMax < (long long)FS_PAD && H.fsOwn + H.fsList < INT32_MAX;
 
-    // ---- 3. per-band halo lists and entries ---------------------------------
-    std::vector<uint16_t> col((size_t)std::max<long long>(nEntries, 1));
-    std::vector<int> code((size_t)std::max<long long>(nEntries, 1));
-    std::vector<std::vector<int>> halo(nBands);
+    // per-band halo lists
+    P.halo.resize(nBands);
     int tooWide = 0;
 #pragma omp parallel for schedule(dynamic, 4) reduction(+ : tooWide)
     for (int b = 0; b < nBands; b++) {
         const int r0 = b * bandRows, r1 = r0 + bandRows;
-        std::vector<int> &h = halo[b];
+        std::vector<int> &h = P.halo[b];
         for (int r = r0; r < r1; r++) {
             int c = iperm[r];
             if (c < 0) continue;
-            for (int f = ownerStart[c]; f < ownerStart[c + 1]; f++) {
-                int t = perm[u[f]];
+            for (int f = g.ownerStart[c]; f < g.ownerStart[c + 1]; f++) {
+                int t = perm[g.u[f]];
                 if (t < r0 || t >= r1) h.push_back(t);
             }
-            for (int k = losortStart[c]; k < losortStart[c + 1]; k++) {
-                int t = perm[l[losort[k]]];
+            for (int k = g.losortStart[c]; k < g.losortStart[c + 1]; k++) {
+                int t = perm[g.l[g.losort[k]]];
                 if (t < r0 || t >= r1) h.push_back(t);
             }
-            for (int k = pfStart[c]; k < pfStart[c + 1]; k++) h.push_back(nPad + pfItem[k]);
+            for (int k = g.pfStart[c]; k < g.pfStart[c + 1]; k++) h.push_back(nPad + g.pfItem[k]);
         }
         std::sort(h.begin(), h.end());
         h.erase(std::unique(h.begin(), h.end()), h.end());
-        if ((long long)bandRows + (long long)h.size() > 65536) {
-            tooWide++;
-            continue;
-        }
-        auto colOf = [&](int t) -> uint16_t {
-            if (t >= r0 && t < r1) return (uint16_t)(t - r0);
-            int pos = (int)(std::lower_bound(h.begin(), h.end(), t) - h.begin());
-            return (uint16_t)(bandRows + pos);
-        };
+        if ((long long)bandRows + (long long)h.size() > 65536) tooWide++;
+    }
+    P.tooWide = tooWide;
+    H.haloStart.assign((size_t)nBands + 1, 0);
+    for (int b = 0; b < nBands; b++) {
+        H.haloStart[b + 1] = H.haloStart[b] + (int)P.halo[b].size();
+        H.maxHalo = std::max(H.maxHalo, (int)P.halo[b].size());
+    }
+    // The check counts two vectors per tile, as when the engine could stage two: the factor is now a margin.  Changing
+    // it changes the band size chosen for poorly clustered meshes.
+    P.tileFits = (size_t)(bandRows + H.maxHalo + 2) * 2 * sizeof(double) <= TILE_BYTES_MAX;
+    return B200LDU_OK;
+}
+
+// ---- 5. face-stream choice ------------------------------------------------------
+// The face stream's CTAs hold the product buffer next to the tile.  It is used where that still leaves as many
+// CTAs per SM as the entry stream's tile alone (large meshes with 512-row bands; not the one-wave bands of mid-size
+// meshes nor GAMG levels with many faces per row).  B200LDU_FACE_STREAM=0 never uses it, =1 whenever it fits.
+bool select_face_stream(const Plan &P)
+{
+    const LayoutHost &H = P.H;
+    const long long tile = ((long long)H.bandRows + H.maxHalo + 1) & ~1ll;
+    const bool fitsSmem = (size_t)(tile + H.fsBufMax) * sizeof(double) <= TILE_BYTES_MAX;
+    if (const char *e = getenv("B200LDU_FACE_STREAM")) {
+        if (!strcmp(e, "0")) return false;
+        if (!strcmp(e, "1")) return P.fsFits && fitsSmem;
+    }
+    return P.fsFits && fitsSmem && ctas_per_sm(tile + H.fsBufMax) >= ctas_per_sm(tile);
+}
+
+// tile column of extended index t (banded row, or nPad + received slot) in band b: its own rows, then its halo list
+uint16_t tile_col(const Plan &P, int b, int t)
+{
+    const int bandRows = P.H.bandRows, r0 = b * bandRows;
+    if (t >= r0 && t < r0 + bandRows) return (uint16_t)(t - r0);
+    const std::vector<int> &h = P.halo[b];
+    return (uint16_t)(bandRows + (std::lower_bound(h.begin(), h.end(), t) - h.begin()));
+}
+
+// ---- 6. entry stream and the concatenated halo lists ------------------------------
+void fill_entry_stream(const Graph &g, const std::vector<int> &perm, Plan &P)
+{
+    LayoutHost &H = P.H;
+    const int bandRows = H.bandRows, slicesPerBand = bandRows / SLICE_ROWS, nPad = H.nPad;
+    const std::vector<int> &iperm = P.iperm;
+    std::vector<uint16_t> &col = H.col;
+    std::vector<int> &code = H.code;
+    col.assign((size_t)std::max<long long>(H.nEntries, 1), 0);
+    code.assign(col.size(), 0);
+#pragma omp parallel for schedule(dynamic, 4)
+    for (int b = 0; b < H.nBands; b++) {
+        const int r0 = b * bandRows;
         for (int sl = 0; sl < slicesPerBand; sl++) {
             int s = b * slicesPerBand + sl;
-            long long base = sliceStart[s];
-            int W = sliceW[s], WL = sliceWL[s];
+            long long base = H.sliceStart[s];
+            int W = H.sliceW[s], WL = H.sliceWL[s];
             for (int q = 0; q < SLICE_ROWS; q++) {
                 int r = s * SLICE_ROWS + q;
                 int c = iperm[r];
                 uint16_t self = (uint16_t)(r - r0);
                 int j = 0;
                 if (c >= 0) {
-                    for (int f = ownerStart[c]; f < ownerStart[c + 1]; f++, j++) {
-                        col[base + (long long)j * SLICE_ROWS + q] = colOf(perm[u[f]]);
+                    for (int f = g.ownerStart[c]; f < g.ownerStart[c + 1]; f++, j++) {
+                        col[base + (long long)j * SLICE_ROWS + q] = tile_col(P, b, perm[g.u[f]]);
                         code[base + (long long)j * SLICE_ROWS + q] = 2 * f;
                     }
-                    for (int k = losortStart[c]; k < losortStart[c + 1]; k++, j++) {
-                        int f = losort[k];
-                        col[base + (long long)j * SLICE_ROWS + q] = colOf(perm[l[f]]);
+                    for (int k = g.losortStart[c]; k < g.losortStart[c + 1]; k++, j++) {
+                        int f = g.losort[k];
+                        col[base + (long long)j * SLICE_ROWS + q] = tile_col(P, b, perm[g.l[f]]);
                         code[base + (long long)j * SLICE_ROWS + q] = 2 * f + 1;
                     }
                 }
@@ -425,9 +467,9 @@ int layout_build(b200ldu_addr *a, const double *centres)
                     code[base + (long long)j * SLICE_ROWS + q] = -1;
                 }
                 if (c >= 0) {
-                    for (int k = pfStart[c]; k < pfStart[c + 1]; k++, j++) {
-                        col[base + (long long)j * SLICE_ROWS + q] = colOf(nPad + pfItem[k]);
-                        code[base + (long long)j * SLICE_ROWS + q] = -2 - pfItem[k];
+                    for (int k = g.pfStart[c]; k < g.pfStart[c + 1]; k++, j++) {
+                        col[base + (long long)j * SLICE_ROWS + q] = tile_col(P, b, nPad + g.pfItem[k]);
+                        code[base + (long long)j * SLICE_ROWS + q] = -2 - g.pfItem[k];
                     }
                 }
                 for (; j < W; j++) {
@@ -436,24 +478,47 @@ int layout_build(b200ldu_addr *a, const double *centres)
                 }
             }
         }
-        if (!fsFits) continue;
-        // face stream: product slot j of row n (slot 0 holds the row's owner-pass sum)
-        auto slotOf = [&](int n, int j) -> uint32_t {
-            const FsSlice &S = fsSlice[n / SLICE_ROWS];
-            return (uint32_t)(S.bufOff + j * SLICE_ROWS + n % SLICE_ROWS);
-        };
+    }
+    H.haloIdx.assign((size_t)std::max(H.haloStart[H.nBands], 1), 0);
+#pragma omp parallel for schedule(static)
+    for (int b = 0; b < H.nBands; b++)
+        std::copy(P.halo[b].begin(), P.halo[b].end(), H.haloIdx.begin() + H.haloStart[b]);
+}
+
+// ---- 7. face stream: owner entries, then each band's list ---------------------------
+void fill_face_stream(const Graph &g, const std::vector<int> &perm, Plan &P)
+{
+    LayoutHost &H = P.H;
+    const int bandRows = H.bandRows, slicesPerBand = bandRows / SLICE_ROWS, nPad = H.nPad;
+    const std::vector<int> &iperm = P.iperm;
+    // nbSlot[f]: position of face f among its neighbour cell's losort faces
+    std::vector<int> nbSlot((size_t)std::max(g.nFaces, 1));
+    for (int c = 0; c < g.nCells; c++)
+        for (int k = g.losortStart[c]; k < g.losortStart[c + 1]; k++) nbSlot[g.losort[k]] = k - g.losortStart[c];
+    std::vector<uint32_t> &fsCT = H.fsCT;
+    std::vector<int> &fsCode = H.fsCode;
+    fsCT.assign((size_t)std::max<long long>(H.fsOwn + H.fsList, 1), 0);
+    fsCode.assign(fsCT.size(), 0);
+    // product slot j of row n (slot 0 holds the row's owner-pass sum)
+    auto slotOf = [&](int n, int j) -> uint32_t {
+        const FsSlice &S = H.fsSlice[n / SLICE_ROWS];
+        return (uint32_t)(S.bufOff + j * SLICE_ROWS + n % SLICE_ROWS);
+    };
+#pragma omp parallel for schedule(dynamic, 4)
+    for (int b = 0; b < H.nBands; b++) {
+        const int r0 = b * bandRows, r1 = r0 + bandRows;
         for (int sl = 0; sl < slicesPerBand; sl++) {
             const int s = b * slicesPerBand + sl;
-            const FsSlice &S = fsSlice[s];
+            const FsSlice &S = H.fsSlice[s];
             const long long base = (long long)S.start64 * SLICE_ROWS;
             for (int q = 0; q < SLICE_ROWS; q++) {
                 const int r = s * SLICE_ROWS + q, c = iperm[r];
                 int j = 0;
                 if (c >= 0) {
-                    for (int f = ownerStart[c]; f < ownerStart[c + 1]; f++, j++) {
-                        const int n = perm[u[f]];
+                    for (int f = g.ownerStart[c]; f < g.ownerStart[c + 1]; f++, j++) {
+                        const int n = perm[g.u[f]];
                         const uint32_t t = (n >= r0 && n < r1) ? slotOf(n, 1 + nbSlot[f]) : FS_NONE;
-                        fsCT[base + (long long)j * SLICE_ROWS + q] = colOf(n) | t << 16;
+                        fsCT[base + (long long)j * SLICE_ROWS + q] = tile_col(P, b, n) | t << 16;
                         fsCode[base + (long long)j * SLICE_ROWS + q] = 2 * f;
                     }
                 }
@@ -463,157 +528,128 @@ int layout_build(b200ldu_addr *a, const double *centres)
                 }
             }
         }
-        int ix = fsListStart[b], ii = fsListIfc[b];
+        int ix = H.fsListStart[b], ii = H.fsListIfc[b];
         for (int r = r0; r < r1; r++) {
             const int c = iperm[r];
             if (c < 0) continue;
-            for (int k = losortStart[c]; k < losortStart[c + 1]; k++) {
-                const int f = losort[k], o = perm[l[f]];
+            for (int k = g.losortStart[c]; k < g.losortStart[c + 1]; k++) {
+                const int f = g.losort[k], o = perm[g.l[f]];
                 if (o >= r0 && o < r1) continue;
-                fsCT[ix] = colOf(o) | slotOf(r, 1 + (k - losortStart[c])) << 16;
+                fsCT[ix] = tile_col(P, b, o) | slotOf(r, 1 + (k - g.losortStart[c])) << 16;
                 fsCode[ix++] = 2 * f + 1;
             }
-            const int wn = fsSlice[r / SLICE_ROWS].wn;
-            for (int k = pfStart[c]; k < pfStart[c + 1]; k++) {
-                fsCT[ii] = colOf(nPad + pfItem[k]) | slotOf(r, 1 + wn + (k - pfStart[c])) << 16;
-                fsCode[ii++] = -2 - pfItem[k];
+            const int wn = H.fsSlice[r / SLICE_ROWS].wn;
+            for (int k = g.pfStart[c]; k < g.pfStart[c + 1]; k++) {
+                fsCT[ii] = tile_col(P, b, nPad + g.pfItem[k]) | slotOf(r, 1 + wn + (k - g.pfStart[c])) << 16;
+                fsCode[ii++] = -2 - g.pfItem[k];
             }
         }
     }
-    if (tooWide) {
-        if (bandRows > SLICE_ROWS) { // retry with narrower bands (see the tile check below)
-            const int saved = g_bandRowsRetry;
-            g_bandRowsRetry = bandRows / 2;
-            int rc = layout_build(a, centres);
-            g_bandRowsRetry = saved;
-            return rc;
-        }
-        b200_set_error("layout_build: %d band(s) of %d rows reference more than 65535 distinct columns",
-                       tooWide, bandRows);
+}
+
+// uploads h and records the allocation in a->layoutMem, which b200ldu_addr_destroy frees
+template <class Ptr, class T>
+int upload(b200ldu_addr *a, Ptr &d, const std::vector<T> &h)
+{
+    T *p = nullptr;
+    const int rc = dev_upload(&p, h);
+    if (p) a->layoutMem.push_back(p);
+    d = p;
+    return rc;
+}
+
+// ---- 8. device path: upload the record, set every layout field of the addressing ----
+int layout_upload(b200ldu_addr *a, const Graph &g, const LayoutHost &H)
+{
+    LayoutDev &L = a->L;
+    TRY(upload(a, L.sliceStart, H.sliceStart));
+    TRY(upload(a, L.sliceW, H.sliceW));
+    TRY(upload(a, L.sliceWL, H.sliceWL));
+    TRY(upload(a, L.col, H.col));
+    TRY(upload(a, a->d_code, H.code));
+    TRY(upload(a, L.haloStart, H.haloStart));
+    TRY(upload(a, L.haloIdx, H.haloIdx));
+    TRY(upload(a, L.perm, a->perm_h));
+    TRY(upload(a, L.iperm, a->iperm_h));
+    TRY(upload(a, L.sendRows, H.sendRows));
+    TRY(upload(a, a->d_l, a->l));
+    TRY(upload(a, a->d_u, a->u));
+    TRY(upload(a, a->d_ownerStart, g.ownerStart));
+    TRY(upload(a, a->d_losort, g.losort));
+    TRY(upload(a, a->d_losortStart, g.losortStart));
+    if (H.hasFs) {
+        TRY(upload(a, L.fsSlice, H.fsSlice));
+        TRY(upload(a, L.fsCT, H.fsCT));
+        TRY(upload(a, a->d_fsCode, H.fsCode));
+        TRY(upload(a, L.fsListStart, H.fsListStart));
+        TRY(upload(a, L.fsListIfc, H.fsListIfc));
+    }
+    L.nCells = g.nCells;
+    L.nPad = H.nPad;
+    L.nBands = H.nBands;
+    L.bandRows = H.bandRows;
+    L.slicesPerBand = H.bandRows / SLICE_ROWS;
+    L.nRecv = H.nRecv;
+    L.maxHalo = H.maxHalo;
+    L.fsBufMax = H.hasFs ? (int)H.fsBufMax : 0;
+    a->nEntries = H.nEntries;
+    a->nHaloTotal = H.haloStart[H.nBands];
+    a->vecLen = ((long long)H.nPad + H.nRecv + 1) & ~1ll;
+    a->hasFs = H.hasFs;
+    a->fsOwn = H.fsOwn;
+    a->fsList = H.fsList;
+    return B200LDU_OK;
+}
+
+} // namespace
+
+int layout_build(b200ldu_addr *a, const double *centres)
+{
+    Graph g{a->nCells, a->nFaces, a->nPatches ? a->patchStart[a->nPatches] : 0, a->l, a->u};
+    TRY(build_csr(g));
+    const std::vector<int> order = renumber(g, centres);
+    a->perm_h.assign(g.nCells, 0);
+    for (int r = 0; r < g.nCells; r++) a->perm_h[order[r]] = r;
+    build_patch_faces(a->faceCells, g);
+
+    int packCtas = 0;
+    for (int p = 0; p < a->nPatches; p++)
+        if (p < (int)a->neighbRank.size() && a->neighbRank[p] >= 0) packCtas += (a->patchStart[p + 1] - a->patchStart[p] + PACK_CHUNK - 1) / PACK_CHUNK;
+    Plan P;
+    for (int bandRows = pick_band_rows(g.nCells, a->ctx ? a->ctx->smCount : 132, packCtas);; bandRows /= 2) {
+        TRY(plan_layout(g, order, a->perm_h, bandRows, P));
+        if (!P.tooWide && P.tileFits) break;
+        // poorly clustered numbering (no cell centres, high-degree graph): narrower bands shrink both the halo and the
+        // tile; the row order is unchanged
+        if (bandRows > SLICE_ROWS) continue;
+        if (P.tooWide)
+            b200_set_error("layout_build: %d band(s) of %d rows reference more than 65535 distinct columns",
+                           P.tooWide, bandRows);
+        else
+            b200_set_error("layout_build: a band of %d rows references %d outside columns: the tile does not fit in "
+                           "shared memory; pass cell centres (or renumber the mesh) so that neighbours are close",
+                           bandRows, P.H.maxHalo);
         return B200LDU_ELAYOUT;
     }
-    std::vector<int> haloStart((size_t)nBands + 1, 0);
-    int maxHalo = 0;
-    for (int b = 0; b < nBands; b++) {
-        haloStart[b + 1] = haloStart[b] + (int)halo[b].size();
-        maxHalo = std::max(maxHalo, (int)halo[b].size());
+    LayoutHost &H = P.H;
+    H.hasFs = select_face_stream(P);
+    fill_entry_stream(g, a->perm_h, P);
+    // a host-only layout keeps the face stream whether or not the engine would use it, so that its structure can be checked
+    if (P.fsFits && (H.hasFs || a->hostOnly)) {
+        fill_face_stream(g, a->perm_h, P);
+    } else { // the record holds a face stream only where it was built
+        H.fsSlice.clear();
+        H.fsListStart.clear();
+        H.fsListIfc.clear();
     }
-    if ((size_t)(bandRows + maxHalo + 2) * 2 * sizeof(double) > TILE_BYTES_MAX) {
-        // poorly clustered numbering (no cell centres, high-degree graph): the halo of a band does not fit
-        // next to its rows in shared memory.  Narrower bands shrink both terms; the ordering is unchanged.
-        if (bandRows > SLICE_ROWS) {
-            const int saved = g_bandRowsRetry;
-            g_bandRowsRetry = bandRows / 2;
-            int rc = layout_build(a, centres);
-            g_bandRowsRetry = saved;
-            return rc;
-        }
-        b200_set_error("layout_build: a band of %d rows references %d outside columns: the tile does not fit in "
-                       "shared memory; pass cell centres (or renumber the mesh) so that neighbours are close",
-                       bandRows, maxHalo);
-        return B200LDU_ELAYOUT;
-    }
-    std::vector<int> haloIdx((size_t)std::max(haloStart[nBands], 1));
-#pragma omp parallel for schedule(static)
-    for (int b = 0; b < nBands; b++)
-        std::copy(halo[b].begin(), halo[b].end(), haloIdx.begin() + haloStart[b]);
-
-    std::vector<int> sendRows(std::max(nRecv, 1));
-    for (int i = 0; i < nRecv; i++) sendRows[i] = perm[a->faceCells[i]];
-
-    // The face stream's CTAs hold the product buffer next to the tile.  It is used where that still leaves as many
-    // CTAs per SM as the entry stream's tile alone (large meshes with 512-row bands; not the one-wave bands of mid-size
-    // meshes nor GAMG levels with many faces per row).  B200LDU_FACE_STREAM=0 never uses it, =1 whenever it fits.
-    {
-        const long long tile = ((long long)bandRows + maxHalo + 1) & ~1ll;
-        const bool fitsSmem = (size_t)(tile + fsBufMax) * sizeof(double) <= TILE_BYTES_MAX;
-        a->hasFs = fsFits && fitsSmem && ctas_per_sm(tile + fsBufMax) >= ctas_per_sm(tile);
-        if (const char *e = getenv("B200LDU_FACE_STREAM")) {
-            if (!strcmp(e, "0")) a->hasFs = false;
-            if (!strcmp(e, "1")) a->hasFs = fsFits && fitsSmem;
-        }
-        a->fsOwn = fsOwn;
-        a->fsList = fsList;
-    }
-
-    a->nEntries = nEntries;
-    a->nHaloTotal = haloStart[nBands];
-    a->vecLen = ((long long)nPad + nRecv + 1) & ~1ll;
-    a->L.nCells = nCells;
-    a->L.nPad = nPad;
-    a->L.nBands = nBands;
-    a->L.bandRows = bandRows;
-    a->L.slicesPerBand = slicesPerBand;
-    a->L.nRecv = nRecv;
-    a->L.maxHalo = maxHalo;
-    if (a->hostOnly) { // structural self-check path (tests): keep the host arrays, no GPU
-        a->dbg_sliceStart.swap(sliceStart);
-        a->dbg_sliceW.swap(sliceW);
-        a->dbg_sliceWL.swap(sliceWL);
-        a->dbg_col.swap(col);
-        a->dbg_code.swap(code);
-        a->dbg_haloStart.swap(haloStart);
-        a->dbg_haloIdx.swap(haloIdx);
-        if (fsFits) { // built whether or not the engine would use it, so that its structure can be checked
-            a->dbg_fsSlice.swap(fsSlice);
-            a->dbg_fsCT.swap(fsCT);
-            a->dbg_fsCode.swap(fsCode);
-            a->dbg_fsListStart.swap(fsListStart);
-            a->dbg_fsListIfc.swap(fsListIfc);
-        }
-        a->L.fsBufMax = (int)fsBufMax;
+    H.sendRows.assign(std::max(g.nRecv, 1), 0);
+    for (int i = 0; i < g.nRecv; i++) H.sendRows[i] = a->perm_h[a->faceCells[i]];
+    a->iperm_h.swap(P.iperm);
+    if (a->hostOnly) { // structural self-check path (tests): keep the host record, no GPU
+        a->host = std::move(H);
         return B200LDU_OK;
     }
-
-    // ---- 4. upload ----------------------------------------------------------
-    TRY(dev_upload(&a->d_sliceStart, sliceStart));
-    TRY(dev_upload(&a->d_sliceW, sliceW));
-    TRY(dev_upload(&a->d_sliceWL, sliceWL));
-    TRY(dev_upload(&a->d_col, col));
-    TRY(dev_upload(&a->d_code, code));
-    TRY(dev_upload(&a->d_haloStart, haloStart));
-    TRY(dev_upload(&a->d_haloIdx, haloIdx));
-    TRY(dev_upload(&a->d_perm, a->perm_h));
-    TRY(dev_upload(&a->d_iperm, a->iperm_h));
-    TRY(dev_upload(&a->d_sendRows, sendRows));
-    TRY(dev_upload(&a->d_l, a->l));
-    TRY(dev_upload(&a->d_u, a->u));
-    TRY(dev_upload(&a->d_ownerStart, ownerStart));
-    TRY(dev_upload(&a->d_losort, losort));
-    TRY(dev_upload(&a->d_losortStart, losortStart));
-    if (a->hasFs) {
-        TRY(dev_upload(&a->d_fsSlice, fsSlice));
-        TRY(dev_upload(&a->d_fsCT, fsCT));
-        TRY(dev_upload(&a->d_fsCode, fsCode));
-        TRY(dev_upload(&a->d_fsListStart, fsListStart));
-        TRY(dev_upload(&a->d_fsListIfc, fsListIfc));
-    }
-
-    LayoutDev &L = a->L;
-    L.fsSlice = a->d_fsSlice;
-    L.fsCT = a->d_fsCT;
-    L.fsListStart = a->d_fsListStart;
-    L.fsListIfc = a->d_fsListIfc;
-    L.fsBufMax = a->hasFs ? (int)fsBufMax : 0;
-    L.nCells = nCells;
-    L.nPad = nPad;
-    L.nBands = nBands;
-    L.bandRows = bandRows;
-    L.slicesPerBand = slicesPerBand;
-    L.nRecv = nRecv;
-    L.maxHalo = maxHalo;
-    L.sliceStart = a->d_sliceStart;
-    L.sliceW = a->d_sliceW;
-    L.sliceWL = a->d_sliceWL;
-    L.col = a->d_col;
-    L.haloStart = a->d_haloStart;
-    L.haloIdx = a->d_haloIdx;
-    L.perm = a->d_perm;
-    L.iperm = a->d_iperm;
-    a->nEntries = nEntries;
-    a->nHaloTotal = haloStart[nBands];
-    a->vecLen = ((long long)nPad + nRecv + 1) & ~1ll;
-    return B200LDU_OK;
+    return layout_upload(a, g, H);
 }
 
 // ---------------------------------------------------------------------------
@@ -654,29 +690,31 @@ extern "C" int b200ldu_layout_debug_create(int nCells, int nFaces, const int *lo
 extern "C" long long b200ldu_layout_debug_get(const b200ldu_addr *a, int what, void *out, long long cap)
 {
     if (!a || !a->hostOnly) return -1;
+    const LayoutHost &H = a->host;
     auto give = [&](const void *src, size_t elem, long long n) -> long long {
         if (out) memcpy(out, src, elem * (size_t)std::min(n, cap));
         return n;
     };
-    int dims[5] = {a->L.nPad, a->L.nBands, a->L.bandRows, a->L.nRecv, a->L.maxHalo};
+    const long long nFs = H.fsCT.empty() ? 0 : H.fsOwn + H.fsList;
+    int dims[5] = {H.nPad, H.nBands, H.bandRows, H.nRecv, H.maxHalo};
     switch (what) {
     case 0: return give(a->perm_h.data(), 4, (long long)a->perm_h.size());
     case 1: return give(a->iperm_h.data(), 4, (long long)a->iperm_h.size());
-    case 2: return give(a->dbg_sliceStart.data(), 8, (long long)a->dbg_sliceStart.size());
-    case 3: return give(a->dbg_sliceW.data(), 2, (long long)a->dbg_sliceW.size());
-    case 4: return give(a->dbg_sliceWL.data(), 2, (long long)a->dbg_sliceWL.size());
-    case 5: return give(a->dbg_col.data(), 2, a->nEntries);
-    case 6: return give(a->dbg_code.data(), 4, a->nEntries);
-    case 7: return give(a->dbg_haloStart.data(), 4, (long long)a->dbg_haloStart.size());
-    case 8: return give(a->dbg_haloIdx.data(), 4, a->nHaloTotal);
+    case 2: return give(H.sliceStart.data(), 8, (long long)H.sliceStart.size());
+    case 3: return give(H.sliceW.data(), 2, (long long)H.sliceW.size());
+    case 4: return give(H.sliceWL.data(), 2, (long long)H.sliceWL.size());
+    case 5: return give(H.col.data(), 2, H.nEntries);
+    case 6: return give(H.code.data(), 4, H.nEntries);
+    case 7: return give(H.haloStart.data(), 4, (long long)H.haloStart.size());
+    case 8: return give(H.haloIdx.data(), 4, H.haloStart[H.nBands]);
     case 9: return give(dims, 4, 5);
-    case 10: return give(a->dbg_fsSlice.data(), 4, 4 * (long long)a->dbg_fsSlice.size());
-    case 11: return give(a->dbg_fsCT.data(), 4, a->dbg_fsCT.empty() ? 0 : a->fsOwn + a->fsList);
-    case 12: return give(a->dbg_fsCode.data(), 4, a->dbg_fsCode.empty() ? 0 : a->fsOwn + a->fsList);
-    case 13: return give(a->dbg_fsListStart.data(), 4, (long long)a->dbg_fsListStart.size());
-    case 14: return give(a->dbg_fsListIfc.data(), 4, (long long)a->dbg_fsListIfc.size());
+    case 10: return give(H.fsSlice.data(), 4, 4 * (long long)H.fsSlice.size());
+    case 11: return give(H.fsCT.data(), 4, nFs);
+    case 12: return give(H.fsCode.data(), 4, nFs);
+    case 13: return give(H.fsListStart.data(), 4, (long long)H.fsListStart.size());
+    case 14: return give(H.fsListIfc.data(), 4, (long long)H.fsListIfc.size());
     case 15: {
-        long long fd[4] = {a->fsOwn, a->fsList, a->L.fsBufMax, a->hasFs ? 1 : 0};
+        long long fd[4] = {H.fsOwn, H.fsList, (int)H.fsBufMax, H.hasFs ? 1 : 0};
         return give(fd, 8, 4);
     }
     }

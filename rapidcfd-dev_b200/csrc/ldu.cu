@@ -199,15 +199,13 @@ extern "C" int b200ldu_addr_destroy(b200ldu_addr *a)
     if (!a) return B200LDU_OK;
     cudaSetDevice(a->ctx->device);
     cudaStreamSynchronize(a->ctx->stream);
-    void *ptrs[] = {a->d_sliceStart, a->d_sliceW, a->d_sliceWL, a->d_col, a->d_code, a->d_haloStart,
-                    a->d_haloIdx, a->d_perm, a->d_iperm, a->d_sendRows, a->d_l, a->d_u,
-                    a->d_ownerStart, a->d_losort, a->d_losortStart, a->d_bFaceCells, a->d_cyclicSrc,
-                    a->d_bCellStart, a->d_bCellFaces, a->d_bCells, a->d_packPatches, a->d_packChunks,
-                    a->d_cCellStart, a->d_cCellFaces, a->d_cFaceCells, a->d_mulesScratch, a->d_fvmScratch[0],
-                    a->d_fvmScratch[1], a->d_fvmScratch[2], a->d_fvmScratch[3], a->d_fsSlice, a->d_fsCT, a->d_fsCode,
-                    a->d_fsListStart, a->d_fsListIfc};
+    void *ptrs[] = {a->d_bFaceCells, a->d_cyclicSrc, a->d_bCellStart, a->d_bCellFaces, a->d_bCells,
+                    a->d_packPatches, a->d_packChunks, a->d_cCellStart, a->d_cCellFaces, a->d_cFaceCells,
+                    a->d_mulesScratch, a->d_fvmScratch[0], a->d_fvmScratch[1], a->d_fvmScratch[2],
+                    a->d_fvmScratch[3]};
     for (void *p : ptrs)
         if (p) cudaFree(p);
+    for (void *p : a->layoutMem) cudaFree(p);
     for (double *p : a->pool)
         if (p) cudaFree(p);
     delete a;
@@ -282,7 +280,7 @@ __global__ void from_banded_kernel(int nCells, const int *__restrict__ iperm,
 
 int to_banded(b200ldu_addr *a, const double *x, double *xb)
 {
-    to_banded_kernel<<<(a->L.nPad + 255) / 256, 256, 0, a->ctx->stream>>>(a->L.nPad, a->d_iperm, x, xb);
+    to_banded_kernel<<<(a->L.nPad + 255) / 256, 256, 0, a->ctx->stream>>>(a->L.nPad, a->L.iperm, x, xb);
     a->ctx->launches++;
     KERNEL_CHECK();
     return B200LDU_OK;
@@ -291,7 +289,7 @@ int to_banded(b200ldu_addr *a, const double *x, double *xb)
 int from_banded(b200ldu_addr *a, const double *xb, double *x)
 {
     // rows [0, nCells) are the real rows (padding sits at the end)
-    from_banded_kernel<<<(a->nCells + 255) / 256, 256, 0, a->ctx->stream>>>(a->nCells, a->d_iperm, xb, x);
+    from_banded_kernel<<<(a->nCells + 255) / 256, 256, 0, a->ctx->stream>>>(a->nCells, a->L.iperm, xb, x);
     a->ctx->launches++;
     KERNEL_CHECK();
     return B200LDU_OK;
@@ -408,7 +406,7 @@ static int own_copy(b200ldu_matrix *m, int k, const double *src, size_t n, const
 int matrix_set_diag(b200ldu_matrix *m, const double *diag_d)
 {
     b200ldu_addr *a = m->a;
-    fill_diag_kernel<<<(unsigned)((a->vecLen + 255) / 256), 256, 0, a->ctx->stream>>>(a->vecLen, a->L.nPad, a->d_iperm,
+    fill_diag_kernel<<<(unsigned)((a->vecLen + 255) / 256), 256, 0, a->ctx->stream>>>(a->vecLen, a->L.nPad, a->L.iperm,
                                                                                       diag_d, m->d_diag, m->d_rD);
     a->ctx->launches++;
     KERNEL_CHECK();
@@ -460,34 +458,28 @@ extern "C" int b200ldu_matrix_set(b200ldu_matrix *m, const double *diag_d, const
             fill_val_kernel<<<(unsigned)((nf + 255) / 256), 256, 0, st>>>(nf, a->d_fsCode, up, lo, bo, m->d_fval, 0);
             a->ctx->launches++;
         }
-        KERNEL_CHECK();
-        m->haveT = false;
-        m->upper_ext = up;
-        m->bou_ext = bo;
-        m->int_ext = in;
-        m->lower_ext = lo;
-        return matrix_set_diag(m, dg);
-    }
-    if (m->d_fval) cudaFree(m->d_fval);
-    m->d_fval = nullptr;
-    size_t nb = sizeof(double) * (size_t)(ne > 0 ? ne : 1);
-    if (!m->d_val) CUDA_TRY(cudaMalloc((void **)&m->d_val, nb));
-    if (needT && (!m->d_valT || m->d_valT == m->d_val)) {
-        m->d_valT = nullptr;
-        CUDA_TRY(cudaMalloc((void **)&m->d_valT, nb));
-    }
-    if (ne > 0) {
-        unsigned g = (unsigned)((ne + 255) / 256);
-        fill_val_kernel<<<g, 256, 0, st>>>(ne, a->d_code, up, lo, bo, m->d_val, 0);
-        a->ctx->launches++;
-        if (needT) {
-            fill_val_kernel<<<g, 256, 0, st>>>(ne, a->d_code, up, lo, in, m->d_valT, 1);
-            a->ctx->launches++;
+    } else {
+        if (m->d_fval) cudaFree(m->d_fval);
+        m->d_fval = nullptr;
+        size_t nb = sizeof(double) * (size_t)(ne > 0 ? ne : 1);
+        if (!m->d_val) CUDA_TRY(cudaMalloc((void **)&m->d_val, nb));
+        if (needT && (!m->d_valT || m->d_valT == m->d_val)) {
+            m->d_valT = nullptr;
+            CUDA_TRY(cudaMalloc((void **)&m->d_valT, nb));
         }
-    }
-    if (!needT) {
-        if (m->d_valT && m->d_valT != m->d_val) cudaFree(m->d_valT);
-        m->d_valT = m->d_val; // A^T == A
+        if (ne > 0) {
+            unsigned g = (unsigned)((ne + 255) / 256);
+            fill_val_kernel<<<g, 256, 0, st>>>(ne, a->d_code, up, lo, bo, m->d_val, 0);
+            a->ctx->launches++;
+            if (needT) {
+                fill_val_kernel<<<g, 256, 0, st>>>(ne, a->d_code, up, lo, in, m->d_valT, 1);
+                a->ctx->launches++;
+            }
+        }
+        if (!needT) {
+            if (m->d_valT && m->d_valT != m->d_val) cudaFree(m->d_valT);
+            m->d_valT = m->d_val; // A^T == A
+        }
     }
     KERNEL_CHECK();
     m->haveT = needT;

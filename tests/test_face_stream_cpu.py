@@ -1,12 +1,11 @@
 """Face stream of symmetric matrices without a GPU: every face is stored once in its owner's row, every product
 for a neighbour row has exactly one slot in its band's shared-memory buffer, and a scalar replay of the engine's
 two passes (owner pass + list, then each row's buffer slots in order) reproduces the oracle's Amul bit for bit."""
-import ctypes as C
 import importlib
-import os
 
 import numpy as np
 import pytest
+from layout_helpers import debug_layout
 
 FS_PAD, FS_NONE = 0xFFFE, 0xFFFF
 
@@ -16,45 +15,6 @@ def capi():
     g = importlib.import_module("__graft_entry__")
     g.build()
     return importlib.import_module("rapidcfd-dev_b200.capi")
-
-
-def _layout(capi, mesh, centres=True, band=None, patches=None):
-    L = capi.lib()
-    L.b200ldu_layout_debug_get.restype = C.c_longlong
-    L.b200ldu_layout_debug_get.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_longlong]
-    L.b200ldu_layout_debug_create.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
-                                              C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p)]
-    L.b200ldu_layout_debug_destroy.argtypes = [C.c_void_p]
-    ps, fc = patches if patches is not None else mesh.patch_start_facecells()
-    ps, fc = np.ascontiguousarray(ps, np.int32), np.ascontiguousarray(fc, np.int32)
-    nP = len(ps) - 1
-    l = np.ascontiguousarray(mesh.lower, np.int32)
-    u = np.ascontiguousarray(mesh.upper, np.int32)
-    cc = np.ascontiguousarray(mesh.cell_centres()) if centres else None
-    h = C.c_void_p()
-    old = os.environ.pop("B200LDU_BAND_ROWS", None)
-    if band:
-        os.environ["B200LDU_BAND_ROWS"] = str(band)
-    try:
-        rc = L.b200ldu_layout_debug_create(mesh.nCells, mesh.nFaces, l.ctypes.data, u.ctypes.data, nP,
-                                           ps.ctypes.data if nP else None, fc.ctypes.data if nP else None,
-                                           cc.ctypes.data if cc is not None else None, C.byref(h))
-    finally:
-        os.environ.pop("B200LDU_BAND_ROWS", None)
-        if old is not None:
-            os.environ["B200LDU_BAND_ROWS"] = old
-    assert rc == 0, L.b200ldu_last_error()
-    out = {}
-    for what, name, dt in [(0, "perm", np.int32), (1, "iperm", np.int32), (7, "haloStart", np.int32),
-                           (8, "haloIdx", np.int32), (9, "dims", np.int32), (10, "fsSlice", np.int32),
-                           (11, "fsCT", np.uint32), (12, "fsCode", np.int32), (13, "fsListStart", np.int32),
-                           (14, "fsListIfc", np.int32), (15, "fsDims", np.int64)]:
-        n = L.b200ldu_layout_debug_get(h, what, None, 0)
-        a = np.zeros(max(n, 1), dtype=dt)
-        L.b200ldu_layout_debug_get(h, what, a.ctypes.data, n)
-        out[name] = a[:n]
-    L.b200ldu_layout_debug_destroy(h)
-    return out
 
 
 class _Fs:
@@ -233,7 +193,7 @@ def _check_replay(orc, meshmod, mesh, lay, coef, patches=None, neighbRank=None, 
                                                ((16, 16, 16), True, 512), ((1, 1, 1), True, None)])
 def test_face_stream_hex(capi, orc, meshmod, dims, centres, band):
     mesh = meshmod.hex_mesh(*dims)
-    lay = _layout(capi, mesh, centres, band)
+    lay = debug_layout(capi, mesh, centres, band)
     _check_structure(mesh, lay)
     coef = meshmod.pressure_laplacian(mesh)
     _check_replay(orc, meshmod, mesh, lay, dict(diag=coef["diag"], upper=coef["upper"]))
@@ -242,7 +202,7 @@ def test_face_stream_hex(capi, orc, meshmod, dims, centres, band):
 def test_face_stream_processor_patches(capi, orc, meshmod):
     for rank in range(4):
         mesh = meshmod.decompose(8, 4, rank)
-        lay = _layout(capi, mesh, True, 64)
+        lay = debug_layout(capi, mesh, True, 64)
         fs = _check_structure(mesh, lay)
         assert fs.nRecv > 0 and np.any(fs.li < fs.ls[1:])
         coef = meshmod.pressure_laplacian(mesh)
@@ -254,7 +214,7 @@ def test_face_stream_processor_patches(capi, orc, meshmod):
 def test_face_stream_cyclic(capi, orc, meshmod):
     from test_oracle_core import _cyclic_case
     m, c, ps, fc, nr, lo, hi = _cyclic_case(meshmod, "P")
-    lay = _layout(capi, m, True, None, patches=(ps, fc))
+    lay = debug_layout(capi, m, True, None, patches=(ps, fc))
     _check_structure(m, lay, patches=(ps, fc))
     _check_replay(orc, meshmod, m, lay, dict(diag=c["diag"], upper=c["upper"], bou=c["bou"]), patches=(ps, fc),
                   neighbRank=nr)
@@ -264,7 +224,7 @@ def test_face_stream_narrowed_bands(capi, orc):
     """A random graph without locality: the builder narrows the bands; the face stream stays exact."""
     from test_layout_cpu import _RandomGraph
     g = _RandomGraph(30000, 6, 1)
-    lay = _layout(capi, g, centres=False, band=16384)
+    lay = debug_layout(capi, g, centres=False, band=16384)
     assert int(lay["dims"][2]) < 16384
     _check_structure(g, lay)
     rng = np.random.default_rng(3)
@@ -280,6 +240,6 @@ def test_face_stream_narrowed_bands(capi, orc):
 def test_face_stream_selection(capi, meshmod):
     """Large meshes use the face stream; its buffer never costs residency against the entry stream's tile."""
     mesh = meshmod.hex_mesh(64)
-    lay = _layout(capi, mesh, True, 512)
+    lay = debug_layout(capi, mesh, True, 512)
     fs = _Fs(lay)
     assert fs.used == 1 and fs.nOwn >= mesh.nFaces

@@ -11,7 +11,8 @@ import numpy as np
 import pytest
 
 from conftest import dense_from_ldu
-from test_layout_cpu import _check_layout, _layout, capi  # noqa: F401  (capi is a fixture)
+from layout_helpers import debug_layout
+from test_layout_cpu import _check_layout, capi  # noqa: F401  (capi is a fixture)
 
 
 @pytest.fixture(scope="module")
@@ -306,7 +307,7 @@ def test_unstructured_case_from_disk_drives_oracle_and_layout(ff, meshmod, orc, 
     assert perf.converged
     np.testing.assert_allclose(psi, xs, atol=1e-6)
     mesh = _AsMesh(pm, g["C"] if centres else None)
-    lay = _layout(capi, mesh, centres=centres, band=64)
+    lay = debug_layout(capi, mesh, centres=centres, band=64)
     _check_layout(mesh, lay)
     nPad, nBands, bandRows, nRecv, maxHalo = [int(x) for x in lay["dims"]]
     assert nBands >= 3 and maxHalo < 4 * bandRows      # the renumbering keeps the bands compact

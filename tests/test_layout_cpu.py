@@ -9,6 +9,7 @@ import re
 
 import numpy as np
 import pytest
+from layout_helpers import debug_layout, debug_lib
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -40,41 +41,6 @@ def test_no_gpu_is_a_loud_error(capi):
     assert b"no CPU fallback" in capi.lib().b200ldu_last_error()
     with pytest.raises(RuntimeError):
         capi.Context(0)
-
-
-def _layout(capi, mesh, centres=True, band=None):
-    L = capi.lib()
-    L.b200ldu_layout_debug_get.restype = C.c_longlong
-    L.b200ldu_layout_debug_get.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_longlong]
-    L.b200ldu_layout_debug_create.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
-                                              C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p)]
-    L.b200ldu_layout_debug_destroy.argtypes = [C.c_void_p]
-    if band:
-        os.environ["B200LDU_BAND_ROWS"] = str(band)
-    else:
-        os.environ.pop("B200LDU_BAND_ROWS", None)
-    ps, fc = mesh.patch_start_facecells()
-    nP = len(ps) - 1
-    l = np.ascontiguousarray(mesh.lower, np.int32)
-    u = np.ascontiguousarray(mesh.upper, np.int32)
-    cc = np.ascontiguousarray(mesh.cell_centres()) if centres else None
-    h = C.c_void_p()
-    rc = L.b200ldu_layout_debug_create(mesh.nCells, mesh.nFaces, l.ctypes.data, u.ctypes.data, nP,
-                                       ps.ctypes.data if nP else None, fc.ctypes.data if nP else None,
-                                       cc.ctypes.data if cc is not None else None, C.byref(h))
-    os.environ.pop("B200LDU_BAND_ROWS", None)
-    assert rc == 0, capi.lib().b200ldu_last_error()
-    out = {}
-    for what, (name, dt) in enumerate([("perm", np.int32), ("iperm", np.int32), ("sliceStart", np.int64),
-                                       ("sliceW", np.uint16), ("sliceWL", np.uint16), ("col", np.uint16),
-                                       ("code", np.int32), ("haloStart", np.int32), ("haloIdx", np.int32),
-                                       ("dims", np.int32)]):
-        n = L.b200ldu_layout_debug_get(h, what, None, 0)
-        a = np.zeros(max(n, 1), dtype=dt)
-        L.b200ldu_layout_debug_get(h, what, a.ctypes.data, n)
-        out[name] = a[:n]
-    L.b200ldu_layout_debug_destroy(h)
-    return out
 
 
 def _check_layout(mesh, lay):
@@ -134,13 +100,13 @@ def _check_layout(mesh, lay):
                                                ((1, 1, 1), True, None), ((5, 1, 1), True, None)])
 def test_layout_structure(capi, meshmod, dims, centres, band):
     mesh = meshmod.hex_mesh(*dims)
-    _check_layout(mesh, _layout(capi, mesh, centres, band))
+    _check_layout(mesh, debug_layout(capi, mesh, centres, band))
 
 
 def test_layout_with_processor_patches(capi, meshmod):
     for rank in range(4):
         mesh = meshmod.decompose(8, 4, rank)
-        lay = _layout(capi, mesh, True, 64)
+        lay = debug_layout(capi, mesh, True, 64)
         assert lay["dims"][3] == sum(len(p.faceCells) for p in mesh.coupled_patches()) > 0
         _check_layout(mesh, lay)
 
@@ -149,7 +115,7 @@ def test_layout_bricks_are_compact(capi, meshmod):
     """32^3 with 512-row bands: Morton tiles of 8x8x8 => every band is one brick and its halo is
     exactly the brick's face-adjacent cells (<= 6*64)."""
     mesh = meshmod.hex_mesh(32)
-    lay = _layout(capi, mesh, True, 512)
+    lay = debug_layout(capi, mesh, True, 512)
     nPad, nBands, bandRows, nRecv, maxHalo = [int(x) for x in lay["dims"]]
     assert bandRows == 512 and nBands == 64
     assert maxHalo <= 6 * 64
@@ -162,12 +128,10 @@ def test_layout_bricks_are_compact(capi, meshmod):
 
 
 def test_layout_rejects_bad_addressing(capi):
-    L = capi.lib()
+    L = debug_lib(capi)
     l = np.array([1, 0], np.int32)  # not owner-sorted
     u = np.array([2, 1], np.int32)
     h = C.c_void_p()
-    L.b200ldu_layout_debug_create.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
-                                              C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p)]
     rc = L.b200ldu_layout_debug_create(3, 2, l.ctypes.data, u.ctypes.data, 0, None, None, None, C.byref(h))
     assert rc == -1
 
@@ -191,11 +155,11 @@ class _RandomGraph:
 
 
 def test_layout_narrows_bands_until_the_tile_fits(capi):
-    """A band's rows + halo columns are staged in shared memory (two vectors at most): when a
+    """A band's rows + halo columns are staged in shared memory (the check allows for two vectors): when a
     numbering without locality makes that tile too large -- or needs more than 65535 columns -- the
     builder halves bandRows until it fits instead of failing at launch time."""
     g = _RandomGraph(30000, 6, 1)
-    lay = _layout(capi, g, centres=False, band=16384)
+    lay = debug_layout(capi, g, centres=False, band=16384)
     nPad, nBands, bandRows, nRecv, maxHalo = [int(x) for x in lay["dims"]]
     assert bandRows < 16384 and (bandRows + maxHalo + 2) * 16 <= 200 * 1024
     _check_layout(g, lay)
