@@ -26,10 +26,10 @@ def pcg_sweep_bytes(info):
     while staging and in finish()."""
     nPad, nE, nH = info["nPadRows"], info["nEntries"], info["nHalo"]
     stream = 12 * (info["fsOwnerSlots"] + info["fsListItems"]) if info.get("faceStream") else 10 * nE
-    # A (PcgAinvOp): own rows read rOld, w, p, psi, rD and write psi, rNew, z; halo reads w, rOld, rD
-    a = 64 * nPad + stream + (4 + 24) * nH
-    # B (PcgAmulOp): own rows read z, pOld, diag and write pNew, w; halo reads z, pOld
-    b = 40 * nPad + stream + (4 + 16) * nH
+    # A (PcgAinvOp): own rows read rOld, w, rD and write rNew, z; halo reads w, rOld, rD
+    a = 40 * nPad + stream + (4 + 24) * nH
+    # B (PcgAmulOp): own rows read z, pOld, psi, diag and write pNew, psi, w; halo reads z, pOld
+    b = 56 * nPad + stream + (4 + 16) * nH
     return a, b
 
 
@@ -68,6 +68,7 @@ def pcg_sweeps(n, iters):
         with open(path) as f:
             trace = json.load(f)
     kern = sorted((e for e in trace.get("traceEvents", []) if e.get("cat") == "kernel"), key=lambda e: e["ts"])
+    # the solve's close (pcg_close_kernel: last alpha, r and sum|r| without the preconditioner) is neither sweep
     which = lambda e: "A" if "PcgAinvOp" in e["name"] else ("B" if "PcgAmulOp" in e["name"] else None)
     dur = {"A": [], "B": []}
     gap = {"A->B": [], "B->A": []}
@@ -85,13 +86,14 @@ def pcg_sweeps(n, iters):
     bytesA, bytesB = pcg_sweep_bytes(info)
     med = lambda v: float(np.median(v)) if v else float("nan")
     rows = []
-    for w, nm, nb in (("A", "PCG sweep A (AINV + r/psi update)", bytesA), ("B", "PCG sweep B (p update + Amul)", bytesB)):
+    for w, nm, nb in (("A", "PCG sweep A (AINV + r update)", bytesA), ("B", "PCG sweep B (psi/p update + Amul)", bytesB)):
         us = med(dur[w])
         rows.append({"kernel": nm, "layout_bytes": int(nb), "us_median": us, "us_min": min(dur[w], default=float("nan")),
                      "launches": len(dur[w]), "GBps": nb / (us * 1e-6) / 1e9})
     out = {"n": n, "iters": iters, "layout": info, "sweeps": rows,
            "gap_us_median": {k: med(v) for k, v in gap.items()}, "gaps": {k: len(v) for k, v in gap.items()},
-           "iteration_us": med(dur["A"]) + med(dur["B"]) + med(gap["A->B"]) + med(gap["B->A"])}
+           "iteration_us": med(dur["A"]) + med(dur["B"]) + med(gap["A->B"]) + med(gap["B->A"]),
+           "close_us_median": med([e["dur"] for e in kern if "pcg_close_kernel" in e["name"]])}
     mat.close()
     addr.close()
     ctx.close()

@@ -15,6 +15,7 @@ struct SolverScalars {
     int nIterations, converged, singular, stop;
     int maxIter, minIter, histCap, nSweeps;
     int bodies; // fused PCG: iteration bodies whose A.p product has been formed
+    int psiBodies; // fused PCG: bodies whose alpha p has been added to psi (bodies - 1 or bodies)
     // fused PCG, deferred scalar steps (DeferredStep): steps completed (low 32 bits) | stop (bit 63), published by CTA 0 of
     // each sweep with one release store and read by every other CTA with one acquire load.  On its own 128-byte line so
     // that the waiting CTAs' polling does not slow down CTA 0's writes to the scalars above.
@@ -391,16 +392,15 @@ struct DeferredStep {
 };
 
 // ---- fused PCG kernels (PCG.C:131-205 regrouped into two matrix sweeps per iteration) ----
-// K_A: applies the solution/residual update of the PREVIOUS body (psi += alpha p,
-// r -= alpha w; alpha from the device scalars) while staging r, then preconditions:
-// z = rD*(r - sum v*(rD*r)[c]); fused sums <z,r> and sum|r|.  r is ping-ponged (other bands
-// read the old halo values), psi is updated in place (own rows only).
+// K_A: applies the residual update of the PREVIOUS body (r -= alpha w; alpha from the
+// device scalars) while staging r, then preconditions: z = rD*(r - sum v*(rD*r)[c]); fused
+// sums <z,r> and sum|r|.  r is ping-ponged (other bands read the old halo values).
 template <class Pre>
 struct PcgAinvOp : OpBase {
     static constexpr bool STAGED = true, LOCAL = true;
     static constexpr int NRED = 2;
-    const double *rOld, *w, *p, *rD;
-    double *rNew, *psi, *z;
+    const double *rOld, *w, *rD;
+    double *rNew, *z;
     const SolverScalars *sc;
     Pre pre; // scalar step of the previous sweep, run in this kernel's prologue
     __device__ __forceinline__ bool prologue(const LayoutDev &) const { return pre.run(); }
@@ -415,13 +415,8 @@ struct PcgAinvOp : OpBase {
         if (sc->bodies > 0) {
             const double alpha = sc->alpha;
             double2 ww = *reinterpret_cast<const double2 *>(w + row);
-            double2 pp = *reinterpret_cast<const double2 *>(p + row);
-            double2 x = *reinterpret_cast<const double2 *>(psi + row);
             r.x = fma(-alpha, ww.x, r.x);
             r.y = fma(-alpha, ww.y, r.y);
-            x.x = fma(alpha, pp.x, x.x);
-            x.y = fma(alpha, pp.y, x.y);
-            *reinterpret_cast<double2 *>(psi + row) = x;
         }
         *reinterpret_cast<double2 *>(rNew + row) = r;
         double2 dd = *reinterpret_cast<const double2 *>(rD + row);
@@ -441,14 +436,15 @@ struct PcgAinvOp : OpBase {
     }
 };
 
-// K_B: forms the new search direction while staging (p = z on the first body, else
-// z + beta p; beta from the device scalars; p ping-ponged), then the row arithmetic of
-// AmulOp<1>: w = A p, fused <w,p>.  The halo send (fused pack CTAs) stages the same p at
-// the patch face cells.
+// K_B: applies the solution update of the PREVIOUS body (psi += alpha pOld, own rows, in
+// place) and forms the new search direction while staging (p = z on the first body, else
+// z + beta p; alpha, beta from the device scalars; p ping-ponged), then the row arithmetic
+// of AmulOp<1>: w = A p, fused <w,p>.  The halo send (fused pack CTAs) stages the same p at
+// the patch face cells: stage() stays free of psi.
 template <class Pre>
 struct PcgAmulOp : AmulOp<1> {
     const double *z, *pOld;
-    double *pNew;
+    double *pNew, *psi;
     const SolverScalars *sc;
     Pre pre; // scalar step of the previous sweep, run in this kernel's prologue
     __device__ __forceinline__ bool prologue(const LayoutDev &) const { return pre.run(); }
@@ -458,14 +454,43 @@ struct PcgAmulOp : AmulOp<1> {
     }
     __device__ __forceinline__ double2 stage_own(int row) const
     {
+        // every load before the first store (the compiler may not move a load past a store to a vector that could
+        // alias it): one memory round trip per row pair, not two.  Costs one 8-byte spill outside the loops; the
+        // sweep is 1 % faster for it (DESIGN §4)
         double2 zz = *reinterpret_cast<const double2 *>(z + row);
         if (sc->bodies > 0) {
-            const double beta = sc->beta;
-            double2 po = *reinterpret_cast<const double2 *>(pOld + row);
+            const double alpha = sc->alpha, beta = sc->beta;
+            const double2 po = *reinterpret_cast<const double2 *>(pOld + row);
+            double2 x = *reinterpret_cast<const double2 *>(psi + row);
             zz.x = fma(beta, po.x, zz.x);
             zz.y = fma(beta, po.y, zz.y);
+            x.x = fma(alpha, po.x, x.x);
+            x.y = fma(alpha, po.y, x.y);
+            *reinterpret_cast<double2 *>(psi + row) = x;
         }
         *reinterpret_cast<double2 *>(pNew + row) = zz;
         return zz;
     }
 };
+
+// Close of the fused PCG: sweep A after the last body, without its preconditioner.  Runs the deferred step B of
+// that body (its alpha) and sums |r| of r = rOld - alpha w into per-band partials grouped exactly as PcgAinvOp's sweep
+// groups them (one CTA per band, lane k on rows 2k, 2k+1 of slices warp, warp + 8, ...), so the final residual keeps
+// every bit; the <z,r> slot is 0.  r is not stored: nothing reads it after the solve.
+template <class Pre>
+__global__ void __launch_bounds__(ENGINE_THREADS) pcg_close_kernel(const LayoutDev L, const double *rOld,
+                                                                    const double *w, const SolverScalars *sc,
+                                                                    double *partials, Pre pre)
+{
+    if (!pre.run()) return;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const double alpha = sc->alpha;
+    double red[2] = {0, 0};
+    for (int sl = warp; sl < L.slicesPerBand; sl += ENGINE_THREADS / 32) {
+        const int row = blockIdx.x * L.bandRows + sl * SLICE_ROWS + 2 * lane;
+        const double2 r = *reinterpret_cast<const double2 *>(rOld + row);
+        const double2 ww = *reinterpret_cast<const double2 *>(w + row);
+        red[1] += fabs(fma(-alpha, ww.x, r.x)) + fabs(fma(-alpha, ww.y, r.y));
+    }
+    block_reduce_store<2, ENGINE_THREADS>(red, partials, blockIdx.x);
+}

@@ -208,13 +208,14 @@ int solve_pcg(Solve &S, int pk)
 
 // ---------------------------------------------------------------------------
 // PCG, fused form: TWO launches per iteration (the reference: 8 Thrust launches + 3 host synchronisations,
-// PCG.C:131-205).  Sweep A (PcgAinvOp) applies the psi/r update of the previous body while staging r,
-// preconditions and reduces <z,r>, sum|r|; sweep B (PcgAmulOp) forms p = z + beta p while staging, multiplies
-// and reduces <Ap,p>.  The scalar step that closes each sweep (sum of the per-band partials in fixed order,
-// cross-rank all-reduce over the peer mailboxes, alpha / beta / convergence test) runs in the prologue of the
-// NEXT sweep's kernel (ops.cuh DeferredStep) -- round 1 spent two one-CTA launches per iteration on it.
-// Same recurrences and per-row arithmetic as solve_pcg; the convergence decision of body k is taken at the
-// start of sweep B of body k+1 (the preconditioner sweep that has then already run only overwrote scratch).
+// PCG.C:131-205).  Sweep A (PcgAinvOp) applies the r update of the previous body while staging r,
+// preconditions and reduces <z,r>, sum|r|; sweep B (PcgAmulOp) applies the psi update of the previous body and
+// forms p = z + beta p while staging, multiplies and reduces <Ap,p>.  The scalar step that closes each sweep
+// (sum of the per-band partials in fixed order, cross-rank all-reduce over the peer mailboxes, alpha / beta /
+// convergence test) runs in the prologue of the NEXT sweep's kernel (ops.cuh DeferredStep) -- round 1 spent two
+// one-CTA launches per iteration on it.  Same recurrences and per-row arithmetic as solve_pcg; the convergence
+// decision of body k is taken at the start of sweep B of body k+1 (the preconditioner sweep that has then already
+// run only overwrote scratch).  A solve that stops there leaves body k's psi update to the close.
 // ---------------------------------------------------------------------------
 // scalar step A of the fused PCG: closes body k-1 (residual, convergence: PCG.C:190-205), then beta of body k
 struct PcgStepA {
@@ -225,6 +226,7 @@ struct PcgStepA {
             end_of_body(s, hist, s->sum[1]);
             if (s->stop) return;
         }
+        s->psiBodies = s->bodies; // the sweep B this step opens adds the latest alpha p to psi
         s->wArAold = s->wArA;
         s->wArA = s->sum[0];
         s->beta = s->wArA / s->wArAold;
@@ -272,40 +274,48 @@ int solve_pcg_fused(Solve &S, int pk)
     const int every = S.c.checkEvery > 0 ? S.c.checkEvery : 8;
     const unsigned mod = 2u * (unsigned)every;
 
+    // diagonal / no preconditioner: sweep A is element-wise; its deferred step runs as CTA 0's prologue too
+    auto sweepAew = [&](long long k, const PreA &preA, int *npA) -> int {
+        const double *rOld = rb[k & 1];
+        double *rNew = rb[(k + 1) & 1];
+        return ew_launch<2>(S.ctx, n2, stop, partA, npA, [=] __device__(int i, double *red) {
+            double2 r = CV2(rOld)[i];
+            if (sc->bodies > 0) {
+                const double alpha = sc->alpha;
+                double2 ww = CV2(w)[i];
+                r.x = fma(-alpha, ww.x, r.x);
+                r.y = fma(-alpha, ww.y, r.y);
+            }
+            V2(rNew)[i] = r;
+            double2 zz = r;
+            if (pk == 1) {
+                double2 d = CV2(rD)[i];
+                zz = make_double2(__dmul_rn(d.x, r.x), __dmul_rn(d.y, r.y));
+            }
+            V2(z)[i] = zz;
+            red[0] += zz.x * r.x + zz.y * r.y;
+            red[1] += fabs(r.x) + fabs(r.y);
+        }, preA);
+    };
+    auto preAFor = [&](long long k) {
+        return PreA{partB, a->L.nBands, sc, gB, pr, (unsigned)(2 * (k % every)), mod, k > 0 ? 1 : 0};
+    };
+
     auto body = [&](long long k) -> int {
         const double *rOld = rb[k & 1], *pPrev = pb[k & 1];
         double *rNew = rb[(k + 1) & 1], *pNew = pb[(k + 1) & 1];
         int npA = a->L.nBands;
-        const PreA preA{partB, a->L.nBands, sc, gB, pr, (unsigned)(2 * (k % every)), mod, k > 0 ? 1 : 0};
+        const PreA preA = preAFor(k);
         if (pk == 2) {
             PcgAinvOp<PreA> op;
             op.stop = stop;
             op.partials = partA;
-            op.rOld = rOld, op.rNew = rNew, op.w = w, op.p = pPrev, op.psi = psi, op.z = z, op.rD = m->d_rD;
+            op.rOld = rOld, op.rNew = rNew, op.w = w, op.z = z, op.rD = m->d_rD;
             op.sc = sc;
             op.pre = preA;
             TRY(engine_launch_m(m, false, op));
         } else {
-            // diagonal / no preconditioner: sweep A is element-wise; its deferred step runs as CTA 0's prologue too
-            TRY(ew_launch<2>(S.ctx, n2, stop, partA, &npA, [=] __device__(int i, double *red) {
-                double2 r = CV2(rOld)[i];
-                if (sc->bodies > 0) {
-                    const double alpha = sc->alpha;
-                    double2 ww = CV2(w)[i], pp = CV2(pPrev)[i], x = CV2(psi)[i];
-                    r.x = fma(-alpha, ww.x, r.x);
-                    r.y = fma(-alpha, ww.y, r.y);
-                    V2(psi)[i] = make_double2(fma(alpha, pp.x, x.x), fma(alpha, pp.y, x.y));
-                }
-                V2(rNew)[i] = r;
-                double2 zz = r;
-                if (pk == 1) {
-                    double2 d = CV2(rD)[i];
-                    zz = make_double2(__dmul_rn(d.x, r.x), __dmul_rn(d.y, r.y));
-                }
-                V2(z)[i] = zz;
-                red[0] += zz.x * r.x + zz.y * r.y;
-                red[1] += fabs(r.x) + fabs(r.y);
-            }, preA));
+            TRY(sweepAew(k, preA, &npA));
         }
         int wait = 0;
         TRY(mat_halo(m, pNew, stop, &wait)); // peer-memory path: nothing is launched, the send is fused
@@ -314,17 +324,41 @@ int solve_pcg_fused(Solve &S, int pk)
         op.stop = stop;
         op.partials = partB;
         op.waitHalo = wait;
-        op.z = z, op.pOld = pPrev, op.pNew = pNew, op.out = w, op.diag = m->d_diag;
+        op.z = z, op.pOld = pPrev, op.pNew = pNew, op.psi = psi, op.out = w, op.diag = m->d_diag;
         op.sc = sc;
         op.pre = preB;
         TRY(engine_launch_m(m, false, op));
         return B200LDU_OK;
     };
-    long long mb = (long long)S.c.maxIter + 1 > S.c.minIter ? (long long)S.c.maxIter + 1 : S.c.minIter;
-    TRY(run_iterations(S, mb + 1, body)); // +1: the last body's update is applied (and judged) by the next sweeps
-    // the loop ends on a decision taken in a prologue (or when the bodies run out): one last scalar step closes
-    // whatever sweep ran last without one -- a no-op once the stop flag is set
-    return B200LDU_OK;
+    const long long mb = (long long)S.c.maxIter + 1 > S.c.minIter ? (long long)S.c.maxIter + 1 : S.c.minIter;
+    TRY(run_iterations(S, mb, body));
+    // Close, enqueued after the loop and never captured: the judgement of body mb-1 always stops the solve, so of the
+    // sweep A that would follow only the deferred step B (alpha of body mb-1), r = rOld - alpha w and sum|r| are
+    // needed; then the final end_of_body.  All three are no-ops once the solve has stopped.  (mb is 0 only for a
+    // negative maxIter: no body ran, nothing to close.)
+    if (mb > 0) {
+        int npA = a->L.nBands;
+        if (pk == 2) {
+            pcg_close_kernel<PreA><<<a->L.nBands, ENGINE_THREADS, 0, S.ctx->stream>>>(a->L, rb[mb & 1], w, sc, partA,
+                                                                                       preAFor(mb));
+            S.ctx->launches++;
+            KERNEL_CHECK();
+        } else {
+            TRY(sweepAew(mb, preAFor(mb), &npA));
+        }
+        TRY(scalar_step_on<2>(S, partA, npA, [=] __device__(SolverScalars *s) { end_of_body(s, hist, s->sum[1]); }));
+    }
+    // The last alpha p that no sweep B added to psi (the solve stopped at a judgement, converged or not): exactly
+    // one update, also after a stop, so the stop flag does not gate it.  p of body j lives in pb[(j + 1) & 1], and the
+    // last alpha is body bodies-1's.
+    const double *p0 = pb[0], *p1 = pb[1];
+    return ew_launch<0>(S.ctx, n2, nullptr, nullptr, nullptr, [=] __device__(int i, double *) {
+        const int j = sc->bodies;
+        if (sc->psiBodies == j) return;
+        const double alpha = sc->alpha;
+        const double2 pp = CV2(j & 1 ? p1 : p0)[i], x = CV2(psi)[i];
+        V2(psi)[i] = make_double2(fma(alpha, pp.x, x.x), fma(alpha, pp.y, x.y));
+    });
 }
 
 // ---------------------------------------------------------------------------
