@@ -186,7 +186,9 @@ long long b200ldu_launch_count(const b200ldu_ctx *ctx);
 /* ---- GAMGAgglomeration (pair agglomeration, cached on the mesh:
  * LDU/solvers/GAMG/GAMGAgglomerations/..., GAMGAgglomeration.C:132-233) ----
  * faceWeights_h: HOST double[nFaces] (faceAreaPairGAMGAgglomeration.C:56-78).
- * forward: in/out pairGAMGAgglomeration::forward_ (static in the reference). */
+ * forward: in/out pairGAMGAgglomeration::forward_ (static in the reference).
+ * a may be a host-only addressing without coupled patches (b200ldu_layout_debug_create): the
+ * hierarchy is then built on the host alone, for nlevels / level_size / restrict_addr, without a GPU. */
 int b200ldu_gamg_create(b200ldu_addr *a, const double *faceWeights_h, int nCellsInCoarsestLevel,
                         int mergeLevels, int *forward, b200ldu_gamg **out);
 int b200ldu_gamg_destroy(b200ldu_gamg *g);

@@ -33,11 +33,22 @@
 
 constexpr int MAX_LEVELS = 50; // GAMGAgglomeration.C:94
 
-struct GamgLevel {
-    int nFine = 0, nFineFaces = 0, nCoarse = 0, nCoarseFaces = 0;
-    std::vector<int> restrictAddr;      // fine cell -> coarse cell (caller orders)
+// One level of the hierarchy as the host stage builds it: the maps from the next finer level and the coarse
+// addressing.  With mergeLevels > 1 it is several pair steps composed (combine).
+struct GamgHostLevel {
+    int nFine = 0, nFineFaces = 0, nCoarse = 0, nCoarseFaces = 0, nFinePF = 0, nCoarsePF = 0;
+    std::vector<int> map;               // fine cell -> coarse cell (caller orders)
     std::vector<int> faceRestrict;      // fine face -> coarse face | -(cell+1)
     std::vector<unsigned char> faceFlip;
+    std::vector<int> cOwner, cNeigh;    // coarse addressing
+    std::vector<int> pfRestrict;        // fine patch face -> coarse patch face
+    std::vector<int> cPatchStart, cFaceCells;
+    std::vector<double> cc;             // coarse centres (empty without fine centres)
+};
+
+struct GamgLevel {
+    int nCoarse = 0, nCoarseFaces = 0;
+    std::vector<int> restrictAddr;      // fine cell -> coarse cell (caller orders)
     b200ldu_addr *addr = nullptr;       // coarse level addressing (banded layout built)
     b200ldu_matrix *mat = nullptr;      // coarse level matrix (values refreshed every solve)
     // device maps, banded vector space
@@ -49,7 +60,7 @@ struct GamgLevel {
     int *d_diagFaceStart = nullptr, *d_diagFace = nullptr;   // coarse cell -> collapsed fine faces ascending
     double *d_diag = nullptr, *d_upper = nullptr, *d_lower = nullptr; // caller-order coarse coefficients
     // coupled patches of the coarse level
-    int nFinePF = 0, nCoarsePF = 0;
+    int nCoarsePF = 0;
     std::vector<int> cPatchStart, cFaceCells;
     int *d_pfChildStart = nullptr, *d_pfChild = nullptr; // coarse patch face -> fine patch faces ascending
     double *d_bou = nullptr, *d_int = nullptr;
@@ -61,6 +72,7 @@ struct b200ldu_gamg {
     b200ldu_addr *finest = nullptr;
     int nLevels = 0;
     std::vector<GamgLevel> lev;
+    std::vector<void *> mem; // every device array the levels' set-up allocated (dev_alloc, upload)
     double *d_inv = nullptr; // this rank's rows of the inverse of the (global) coarsest matrix
     int invN = 0;            // global size of the coarsest system
     // multi-rank coarsest solve
@@ -198,25 +210,261 @@ static void csr_from_map(const std::vector<int> &map, int nTargets, std::vector<
         if (map[i] >= 0) items[cur[map[i]]++] = i;
 }
 
-static void level_free(GamgLevel &L)
+// continueAgglomerating (GAMGAgglomeration.C:72-84): and-reduced over the ranks (ctx null: one rank)
+static int continue_vote(b200ldu_ctx *ctx, bool mine, bool &cont)
 {
-    void *ptrs[] = {L.d_childStart, L.d_child, L.d_pmap, L.d_cellChildStart, L.d_cellChild, L.d_faceChildStart,
-                    L.d_faceChild, L.d_diagFaceStart, L.d_diagFace, L.d_diag, L.d_upper, L.d_lower,
-                    L.corr, L.src, L.tmp, L.acf, L.pre, L.d_pfChildStart, L.d_pfChild, L.d_bou, L.d_int};
-    for (void *p : ptrs)
-        if (p) cudaFree(p);
-    if (L.mat) b200ldu_matrix_destroy(L.mat);
-    if (L.addr) b200ldu_addr_destroy(L.addr);
+    double votes = mine ? 0.0 : 1.0;
+    std::vector<double> all(ctx ? (size_t)ctx->nRanks : 1, votes);
+    if (ctx) TRY(comm_allgather_host(ctx, &votes, 1, all.data()));
+    double stopVotes = 0;
+    for (double v : all) stopVotes += v;
+    cont = !(stopVotes > 0);
+    return B200LDU_OK;
+}
+
+// coarse centres = mean of the children (only used to pick the band renumbering)
+static void coarse_centres(const std::vector<double> &centres, GamgHostLevel &H)
+{
+    if (centres.empty()) return;
+    H.cc.assign((size_t)3 * H.nCoarse, 0.0);
+    std::vector<int> cn(H.nCoarse, 0);
+    for (int c = 0; c < H.nFine; c++) {
+        for (int k = 0; k < 3; k++) H.cc[3 * (size_t)H.map[c] + k] += centres[3 * (size_t)c + k];
+        cn[H.map[c]]++;
+    }
+    for (int C = 0; C < H.nCoarse; C++)
+        for (int k = 0; k < 3; k++) H.cc[3 * (size_t)C + k] /= cn[C];
+}
+
+// processor / cyclic interfaces of the coarse level (processorGAMGInterface.C:60-140, cyclicGAMGInterface.C:70-150):
+// unique (master cell, slave cell) pairs in order of first appearance along every fine patch
+static int coarse_patches(const b200ldu_addr *a, const std::vector<int> &fPatchStart, const std::vector<int> &fFaceCells,
+                          GamgHostLevel &H)
+{
+    const int nPatches = a->nPatches;
+    H.nFinePF = nPatches ? fPatchStart[nPatches] : 0;
+    H.pfRestrict.assign(std::max(H.nFinePF, 1), 0);
+    H.cPatchStart.assign((size_t)nPatches + 1, 0);
+    if (!nPatches) return B200LDU_OK;
+    std::vector<int> sendMap(H.nFinePF), nbrMap(H.nFinePF);
+    for (int i = 0; i < H.nFinePF; i++) sendMap[i] = H.map[fFaceCells[i]];
+    TRY(comm_exchange_patch_ints(a->ctx, nPatches, fPatchStart.data(), a->neighbRank.data(), sendMap.data(),
+                                 nbrMap.data()));
+    int nC = 0;
+    for (int p = 0; p < nPatches; p++) {
+        const int nb = a->neighbRank[p], me = a->ctx->rank;
+        // master side first so that both sides enumerate the same pairs: the lower rank of a processor
+        // patch, the owner (= lower patch index) of a cyclic pair (cyclicGAMGInterface.C:104-127)
+        const bool master = nb >= 0 ? (me < nb) : (p < -nb - 1);
+        H.cPatchStart[p] = nC;
+        std::vector<std::pair<int, int>> pairs;
+        for (int i = fPatchStart[p]; i < fPatchStart[p + 1]; i++) {
+            std::pair<int, int> pr = master ? std::make_pair(sendMap[i], nbrMap[i])
+                                            : std::make_pair(nbrMap[i], sendMap[i]);
+            int found = -1;
+            for (int k = (int)pairs.size() - 1; k >= 0; k--)
+                if (pairs[k] == pr) {
+                    found = k;
+                    break;
+                }
+            if (found < 0) {
+                found = (int)pairs.size();
+                pairs.push_back(pr);
+                H.cFaceCells.push_back(sendMap[i]);
+            }
+            H.pfRestrict[i] = nC + found;
+        }
+        nC += (int)pairs.size();
+    }
+    H.cPatchStart[nPatches] = nC;
+    H.nCoarsePF = nC;
+    return B200LDU_OK;
+}
+
+// restrictFaceField of the weights for the next step (pairGAMGAgglomerate.C:86-107)
+static void restrict_weights(const GamgHostLevel &H, std::vector<double> &w)
+{
+    std::vector<double> cw(H.nCoarseFaces, 0.0);
+    for (int f = 0; f < H.nFineFaces; f++)
+        if (H.faceRestrict[f] >= 0) cw[H.faceRestrict[f]] += w[f];
+    w.swap(cw);
+}
+
+// combineLevels (GAMGAgglomerateLduAddressing.C:606-765): fold step N (built on the coarse side
+// of P) into P.  The flip of a composed face is the flip of the second step alone, as in the
+// reference (:631); a face that collapses into a cell carries no flip.
+static void combine(GamgHostLevel &P, GamgHostLevel &N)
+{
+    for (int f = 0; f < P.nFineFaces; f++) {
+        if (P.faceRestrict[f] >= 0) {
+            const int mid = P.faceRestrict[f];
+            P.faceRestrict[f] = N.faceRestrict[mid];
+            P.faceFlip[f] = N.faceFlip[mid];
+        } else {
+            P.faceRestrict[f] = -N.map[-P.faceRestrict[f] - 1] - 1;
+            P.faceFlip[f] = 0;
+        }
+    }
+    for (int c = 0; c < P.nFine; c++) P.map[c] = N.map[P.map[c]];
+    for (int i = 0; i < P.nFinePF; i++) P.pfRestrict[i] = N.pfRestrict[P.pfRestrict[i]];
+    P.nCoarse = N.nCoarse;
+    P.nCoarseFaces = N.nCoarseFaces;
+    P.nCoarsePF = N.nCoarsePF;
+    P.cOwner.swap(N.cOwner);
+    P.cNeigh.swap(N.cNeigh);
+    P.cPatchStart.swap(N.cPatchStart);
+    P.cFaceCells.swap(N.cFaceCells);
+    P.cc.swap(N.cc);
+}
+
+// Host stage: the whole hierarchy (pairGAMGAgglomerate.C:46-117).  Every pair step maps the coarse side of the last
+// level (the finest addressing at first); with mergeLevels > 1 consecutive steps fold into one level.
+static int agglomerate(const b200ldu_addr *a, const double *faceWeights_h, int nCellsInCoarsestLevel, int mergeLevels,
+                       bool &forward, std::vector<GamgHostLevel> &levels)
+{
+    b200ldu_ctx *ctx = a->hostOnly ? nullptr : a->ctx;
+    std::vector<double> w(faceWeights_h, faceWeights_h + a->nFaces);
+    for (int nPairLevels = 0; (int)levels.size() < MAX_LEVELS - 1; nPairLevels++) {
+        const GamgHostLevel *F = levels.empty() ? nullptr : &levels.back();
+        const std::vector<int> &lo = F ? F->cOwner : a->l, &up = F ? F->cNeigh : a->u;
+        GamgHostLevel H;
+        H.nFine = F ? F->nCoarse : a->nCells;
+        H.nFineFaces = (int)lo.size();
+        pair_agglomerate(H.nFine, lo, up, w, forward, H.map, H.nCoarse);
+        bool cont = false;
+        TRY(continue_vote(ctx, H.nCoarse >= nCellsInCoarsestLevel, cont));
+        if (!cont) break;
+        coarse_addressing(lo, up, H.map, H.nCoarse, H.cOwner, H.cNeigh, H.faceRestrict, H.faceFlip);
+        H.nCoarseFaces = (int)H.cOwner.size();
+        coarse_centres(F ? F->cc : a->centres_h, H);
+        TRY(coarse_patches(a, F ? F->cPatchStart : a->patchStart, F ? F->cFaceCells : a->faceCells, H));
+        restrict_weights(H, w);
+        if (nPairLevels % mergeLevels) // pairGAMGAgglomerate.C:110-117
+            combine(levels.back(), H);
+        else
+            levels.push_back(std::move(H));
+    }
+    return B200LDU_OK;
+}
+
+// coarsest level across the ranks: sizes, offsets and the neighbour-side cell of every
+// coarsest processor-patch face (columns of the global matrix, LUscalarMatrix.C:201-270)
+static int coarsest_setup(b200ldu_gamg *g, const b200ldu_addr *a, const GamgHostLevel &LC)
+{
+    const int R = a->ctx->nRanks;
+    if (R == 1 && !a->nPatches) return B200LDU_OK;
+    double mine = LC.nCoarse;
+    std::vector<double> all(R);
+    TRY(comm_allgather_host(a->ctx, &mine, 1, all.data()));
+    g->coarsestCounts.resize(R);
+    g->coarsestOffs.assign(R + 1, 0);
+    g->nMaxCoarsest = 0;
+    for (int r = 0; r < R; r++) {
+        g->coarsestCounts[r] = (int)all[r];
+        g->coarsestOffs[r + 1] = g->coarsestOffs[r] + g->coarsestCounts[r];
+        g->nMaxCoarsest = std::max(g->nMaxCoarsest, g->coarsestCounts[r]);
+    }
+    if (R > 1 && g->nMaxCoarsest > P2P_GMAX) {
+        b200_set_error("GAMG: coarsest level has %d cells on one rank; the multi-rank direct solve "
+                       "supports up to %d (lower nCellsInCoarsestLevel)", g->nMaxCoarsest, P2P_GMAX);
+        return B200LDU_EINVAL;
+    }
+    if (a->nPatches) {
+        g->coarsestNbrCell.resize(std::max(LC.nCoarsePF, 1));
+        TRY(comm_exchange_patch_ints(a->ctx, a->nPatches, LC.cPatchStart.data(), a->neighbRank.data(),
+                                     LC.cFaceCells.data(), g->coarsestNbrCell.data()));
+    }
+    return B200LDU_OK;
+}
+
+// Device stage of one level: its addressing (banded layout and halo set-up), matrix, maps and vectors.  fineAddr is
+// the addressing of the next finer level.  A host-only hierarchy keeps the restrict map and the sizes alone.
+static int level_upload(b200ldu_gamg *g, const b200ldu_addr *fineAddr, GamgHostLevel &&H)
+{
+    const b200ldu_addr *a = g->finest;
+    g->lev.emplace_back();
+    GamgLevel &L = g->lev.back();
+    L.nCoarse = H.nCoarse;
+    L.nCoarseFaces = H.nCoarseFaces;
+    L.nCoarsePF = H.nCoarsePF;
+    L.restrictAddr = std::move(H.map);
+    L.cPatchStart = std::move(H.cPatchStart);
+    L.cFaceCells = std::move(H.cFaceCells);
+    if (a->hostOnly) return B200LDU_OK;
+    const int nPatches = a->nPatches, nCoarse = H.nCoarse;
+    TRY(b200ldu_addr_create(a->ctx, nCoarse, H.nCoarseFaces, H.cOwner.data(), H.cNeigh.data(), nPatches,
+                            nPatches ? L.cPatchStart.data() : nullptr, nPatches ? L.cFaceCells.data() : nullptr,
+                            nPatches ? a->neighbRank.data() : nullptr, H.cc.empty() ? nullptr : H.cc.data(), &L.addr));
+    std::vector<void *> &mem = g->mem;
+    if (nPatches) {
+        std::vector<int> ps, pi;
+        csr_from_map(H.pfRestrict, H.nCoarsePF, ps, pi);
+        TRY(upload(mem, L.d_pfChildStart, ps));
+        TRY(upload(mem, L.d_pfChild, pi));
+        TRY(dev_alloc(mem, L.d_bou, H.nCoarsePF));
+        TRY(dev_alloc(mem, L.d_int, H.nCoarsePF));
+    }
+    TRY(b200ldu_matrix_create(L.addr, &L.mat));
+    // caller order: coarse cell -> fine cells ascending
+    std::vector<int> cs, ci;
+    csr_from_map(L.restrictAddr, nCoarse, cs, ci);
+    TRY(upload(mem, L.d_cellChildStart, cs));
+    TRY(upload(mem, L.d_cellChild, ci));
+    // banded: coarse row -> fine rows, fine row -> coarse row
+    const std::vector<int> &finePerm = fineAddr->perm_h, &fiperm = fineAddr->iperm_h;
+    const std::vector<int> &cperm = L.addr->perm_h, &ciperm = L.addr->iperm_h;
+    const int nPadC = L.addr->L.nPad, nPadF = fineAddr->L.nPad;
+    std::vector<int> bs((size_t)nPadC + 1, 0), bi(std::max(H.nFine, 1));
+    for (int R = 0; R < nPadC; R++) {
+        int C = ciperm[R];
+        int cntC = C >= 0 ? cs[C + 1] - cs[C] : 0;
+        bs[R + 1] = bs[R] + cntC;
+        for (int k = 0; k < cntC; k++) bi[bs[R] + k] = finePerm[ci[cs[C] + k]];
+    }
+    std::vector<int> pm(nPadF, -1);
+    for (int q = 0; q < nPadF; q++)
+        if (fiperm[q] >= 0) pm[q] = cperm[L.restrictAddr[fiperm[q]]];
+    TRY(upload(mem, L.d_childStart, bs));
+    TRY(upload(mem, L.d_child, bi));
+    TRY(upload(mem, L.d_pmap, pm));
+    // face maps (caller order): coarse face -> (fine face << 1 | flip), coarse cell -> collapsed fine faces
+    std::vector<int> fmap(H.nFineFaces), dmap(H.nFineFaces);
+    for (int f = 0; f < H.nFineFaces; f++) {
+        fmap[f] = H.faceRestrict[f] >= 0 ? H.faceRestrict[f] : -1;
+        dmap[f] = H.faceRestrict[f] < 0 ? -1 - H.faceRestrict[f] : -1;
+    }
+    std::vector<int> fs, fi, ds, di;
+    csr_from_map(fmap, H.nCoarseFaces, fs, fi);
+    csr_from_map(dmap, nCoarse, ds, di);
+    for (int k = 0; k < fs[H.nCoarseFaces]; k++) fi[k] = (fi[k] << 1) | (H.faceFlip[fi[k]] ? 1 : 0);
+    TRY(upload(mem, L.d_faceChildStart, fs));
+    TRY(upload(mem, L.d_faceChild, fi));
+    TRY(upload(mem, L.d_diagFaceStart, ds));
+    TRY(upload(mem, L.d_diagFace, di));
+    TRY(dev_alloc(mem, L.d_diag, nCoarse));
+    TRY(dev_alloc(mem, L.d_upper, H.nCoarseFaces));
+    TRY(dev_alloc(mem, L.d_lower, H.nCoarseFaces));
+    for (double **v : {&L.corr, &L.src, &L.tmp, &L.acf, &L.pre}) {
+        TRY(dev_alloc(mem, *v, L.addr->vecLen));
+        CUDA_TRY(cudaMemsetAsync(*v, 0, sizeof(double) * (size_t)L.addr->vecLen, a->ctx->stream));
+    }
+    return B200LDU_OK;
 }
 
 extern "C" int b200ldu_gamg_destroy(b200ldu_gamg *g)
 {
     if (!g) return B200LDU_OK;
-    cudaSetDevice(g->finest->ctx->device);
-    cudaStreamSynchronize(g->finest->ctx->stream);
-    for (auto &L : g->lev) level_free(L);
-    if (g->d_inv) cudaFree(g->d_inv);
-    if (g->d_gatherAll) cudaFree(g->d_gatherAll);
+    if (!g->finest->hostOnly) {
+        cudaSetDevice(g->finest->ctx->device);
+        cudaStreamSynchronize(g->finest->ctx->stream);
+        for (GamgLevel &L : g->lev) {
+            if (L.mat) b200ldu_matrix_destroy(L.mat);
+            if (L.addr) b200ldu_addr_destroy(L.addr);
+        }
+        for (void *p : g->mem) cudaFree(p);
+        if (g->d_inv) cudaFree(g->d_inv);
+        if (g->d_gatherAll) cudaFree(g->d_gatherAll);
+    }
     delete g;
     return B200LDU_OK;
 }
@@ -229,280 +477,34 @@ extern "C" int b200ldu_gamg_create(b200ldu_addr *a, const double *faceWeights_h,
         b200_set_error("GAMG: mergeLevels must be >= 1");
         return B200LDU_EINVAL;
     }
+    if (a->hostOnly && a->nPatches) {
+        b200_set_error("GAMG: a host-only addressing has no neighbour ranks; coupled patches need b200ldu_addr_create");
+        return B200LDU_EINVAL;
+    }
     for (int p = 0; p < a->nPatches; p++)
         if (a->neighbRank[p] == a->ctx->rank && a->ctx->nRanks > 1) {
             b200_set_error("GAMG: patch %d names this rank as its neighbour; cyclic patches are declared with neighbRank = -(partnerPatch + 1)", p);
             return B200LDU_EINVAL;
         }
-    CUDA_TRY(cudaSetDevice(a->ctx->device));
+    if (!a->hostOnly) CUDA_TRY(cudaSetDevice(a->ctx->device));
+    bool forward = forwardInOut ? (*forwardInOut != 0) : true; // pairGAMGAgglomeration.C:33
+    // Every host collective comes first (the votes and patch exchanges of the pairing, then the coarsest-level
+    // all-gather and exchange), the per-level addressing set-up with its own collectives after them.  Every rank
+    // runs the same sequence -- the and-reduced votes give all ranks the same number of levels -- so the
+    // collectives match.
+    std::vector<GamgHostLevel> H;
+    int rc = agglomerate(a, faceWeights_h, nCellsInCoarsestLevel, mergeLevels, forward, H);
+    if (forwardInOut) *forwardInOut = forward ? 1 : 0;
     b200ldu_gamg *g = new b200ldu_gamg();
     g->finest = a;
-    bool forward = forwardInOut ? (*forwardInOut != 0) : true; // pairGAMGAgglomeration.C:33
-    std::vector<int> lo = a->l, up = a->u;
-    std::vector<int> fPatchStart = a->patchStart, fFaceCells = a->faceCells; // coupled patches of the fine level
-    const int nPatches = a->nPatches;
-    std::vector<double> w(faceWeights_h, faceWeights_h + a->nFaces);
-    std::vector<double> centres = a->centres_h;
-    int nFine = a->nCells;
-    int rc = B200LDU_OK;
-
-    // One pairing step on the host (pairGAMGAgglomerate.C:46-107): maps from the current fine
-    // level to the next coarser one.  With mergeLevels > 1 consecutive steps are composed
-    // (combineLevels) before the device structures of the level are built.
-    struct HostStep {
-        int nFine = 0, nFineFaces = 0, nCoarse = 0, nCoarseFaces = 0, nFinePF = 0, nCoarsePF = 0;
-        std::vector<int> map, faceRestrict, cOwner, cNeigh, pfRestrict, cPatchStart, cFaceCells;
-        std::vector<unsigned char> faceFlip;
-        std::vector<double> cc;
-    };
-
-    // build the device side of a finished level
-    auto finalize = [&](HostStep &H) -> int {
-        g->lev.emplace_back();
-        GamgLevel &L = g->lev.back();
-        b200ldu_addr *fineAddr = g->lev.size() >= 2 ? g->lev[g->lev.size() - 2].addr : a;
-        const std::vector<int> &finePerm = fineAddr->perm_h, &fiperm = fineAddr->iperm_h;
-        L.nFine = H.nFine;
-        L.nFineFaces = H.nFineFaces;
-        L.nCoarse = H.nCoarse;
-        L.nCoarseFaces = H.nCoarseFaces;
-        L.nFinePF = H.nFinePF;
-        L.nCoarsePF = H.nCoarsePF;
-        L.restrictAddr.swap(H.map);
-        L.faceRestrict.swap(H.faceRestrict);
-        L.faceFlip.swap(H.faceFlip);
-        L.cPatchStart.swap(H.cPatchStart);
-        L.cFaceCells.swap(H.cFaceCells);
-        const std::vector<int> &map = L.restrictAddr;
-        const int nCoarse = L.nCoarse, nFineL = L.nFine;
-        int r = b200ldu_addr_create(a->ctx, nCoarse, L.nCoarseFaces, H.cOwner.data(), H.cNeigh.data(), nPatches,
-                                    nPatches ? L.cPatchStart.data() : nullptr, nPatches ? L.cFaceCells.data() : nullptr,
-                                    nPatches ? a->neighbRank.data() : nullptr, H.cc.empty() ? nullptr : H.cc.data(),
-                                    &L.addr);
-        if (r != B200LDU_OK) return r;
-        if (nPatches) {
-            std::vector<int> ps, pi;
-            csr_from_map(H.pfRestrict, L.nCoarsePF, ps, pi);
-            TRY(dev_upload(&L.d_pfChildStart, ps));
-            TRY(dev_upload(&L.d_pfChild, pi));
-            if (cudaMalloc((void **)&L.d_bou, sizeof(double) * (size_t)std::max(L.nCoarsePF, 1)) != cudaSuccess ||
-                cudaMalloc((void **)&L.d_int, sizeof(double) * (size_t)std::max(L.nCoarsePF, 1)) != cudaSuccess) {
-                b200_set_error("GAMG: out of device memory");
-                return B200LDU_ECUDA;
-            }
-        }
-        TRY(b200ldu_matrix_create(L.addr, &L.mat));
-        // ---- device maps ----
-        {
-            std::vector<int> cs, ci;
-            csr_from_map(map, nCoarse, cs, ci); // coarse cell -> fine cells ascending
-            TRY(dev_upload(&L.d_cellChildStart, cs));
-            TRY(dev_upload(&L.d_cellChild, ci));
-            // banded versions
-            const std::vector<int> &cperm = L.addr->perm_h, &ciperm = L.addr->iperm_h;
-            const int nPadC = L.addr->L.nPad, nPadF = fineAddr->L.nPad;
-            std::vector<int> bs((size_t)nPadC + 1, 0), bi(std::max(nFineL, 1));
-            for (int R = 0; R < nPadC; R++) {
-                int C = ciperm[R];
-                int cntC = C >= 0 ? cs[C + 1] - cs[C] : 0;
-                bs[R + 1] = bs[R] + cntC;
-                for (int k = 0; k < cntC; k++) bi[bs[R] + k] = finePerm[ci[cs[C] + k]];
-            }
-            std::vector<int> pm(nPadF, -1);
-            for (int q = 0; q < nPadF; q++)
-                if (fiperm[q] >= 0) pm[q] = cperm[map[fiperm[q]]];
-            TRY(dev_upload(&L.d_childStart, bs));
-            TRY(dev_upload(&L.d_child, bi));
-            TRY(dev_upload(&L.d_pmap, pm));
-            // face maps (caller order)
-            std::vector<int> fmap(L.nFineFaces), dmap(L.nFineFaces);
-            for (int f = 0; f < L.nFineFaces; f++) {
-                fmap[f] = L.faceRestrict[f] >= 0 ? L.faceRestrict[f] : -1;
-                dmap[f] = L.faceRestrict[f] < 0 ? -1 - L.faceRestrict[f] : -1;
-            }
-            std::vector<int> fs, fi, ds, di;
-            csr_from_map(fmap, L.nCoarseFaces, fs, fi);
-            csr_from_map(dmap, nCoarse, ds, di);
-            for (int k = 0; k < fs[L.nCoarseFaces]; k++) fi[k] = (fi[k] << 1) | (L.faceFlip[fi[k]] ? 1 : 0);
-            TRY(dev_upload(&L.d_faceChildStart, fs));
-            TRY(dev_upload(&L.d_faceChild, fi));
-            TRY(dev_upload(&L.d_diagFaceStart, ds));
-            TRY(dev_upload(&L.d_diagFace, di));
-        }
-        size_t nf = (size_t)std::max(L.nCoarseFaces, 1);
-        if (cudaMalloc((void **)&L.d_diag, sizeof(double) * (size_t)nCoarse) != cudaSuccess ||
-            cudaMalloc((void **)&L.d_upper, sizeof(double) * nf) != cudaSuccess ||
-            cudaMalloc((void **)&L.d_lower, sizeof(double) * nf) != cudaSuccess) {
-            b200_set_error("GAMG: out of device memory");
-            return B200LDU_ECUDA;
-        }
-        for (double **v : {&L.corr, &L.src, &L.tmp, &L.acf, &L.pre}) TRY(addr_alloc_vec(L.addr, v));
-        return B200LDU_OK;
-    };
-
-    // combineLevels (GAMGAgglomerateLduAddressing.C:606-765): fold step N (built on the coarse side
-    // of P) into P.  The flip of a composed face is the flip of the second step alone, as in the
-    // reference (:631); a face that collapses into a cell carries no flip.
-    auto combine = [&](HostStep &P, HostStep &N) {
-        for (int f = 0; f < P.nFineFaces; f++) {
-            if (P.faceRestrict[f] >= 0) {
-                const int mid = P.faceRestrict[f];
-                P.faceRestrict[f] = N.faceRestrict[mid];
-                P.faceFlip[f] = N.faceFlip[mid];
-            } else {
-                P.faceRestrict[f] = -N.map[-P.faceRestrict[f] - 1] - 1;
-                P.faceFlip[f] = 0;
-            }
-        }
-        for (int c = 0; c < P.nFine; c++) P.map[c] = N.map[P.map[c]];
-        for (int i = 0; i < P.nFinePF; i++) P.pfRestrict[i] = N.pfRestrict[P.pfRestrict[i]];
-        P.nCoarse = N.nCoarse;
-        P.nCoarseFaces = N.nCoarseFaces;
-        P.nCoarsePF = N.nCoarsePF;
-        P.cOwner.swap(N.cOwner);
-        P.cNeigh.swap(N.cNeigh);
-        P.cPatchStart.swap(N.cPatchStart);
-        P.cFaceCells.swap(N.cFaceCells);
-        P.cc.swap(N.cc);
-    };
-
-    HostStep pend;
-    bool havePend = false;
-    int nPairLevels = 0;
-    while ((int)g->lev.size() + (havePend ? 1 : 0) < MAX_LEVELS - 1) {
-        HostStep H;
-        int nCoarse = -1;
-        pair_agglomerate(nFine, lo, up, w, forward, H.map, nCoarse);
-        // continueAgglomerating (GAMGAgglomeration.C:72-84): and-reduced over the ranks
-        {
-            double votes = (nCoarse >= nCellsInCoarsestLevel) ? 0.0 : 1.0;
-            std::vector<double> all((size_t)a->ctx->nRanks, 0.0);
-            rc = comm_allgather_host(a->ctx, &votes, 1, all.data());
-            if (rc != B200LDU_OK) break;
-            double stopVotes = 0;
-            for (double v : all) stopVotes += v;
-            if (stopVotes > 0) break;
-        }
-        H.nFine = nFine;
-        H.nFineFaces = (int)lo.size();
-        H.nCoarse = nCoarse;
-        coarse_addressing(lo, up, H.map, nCoarse, H.cOwner, H.cNeigh, H.faceRestrict, H.faceFlip);
-        H.nCoarseFaces = (int)H.cOwner.size();
-        // coarse centres = mean of the children (only used to pick the band renumbering)
-        if (!centres.empty()) {
-            H.cc.assign((size_t)3 * nCoarse, 0.0);
-            std::vector<int> cn(nCoarse, 0);
-            for (int c = 0; c < nFine; c++) {
-                for (int k = 0; k < 3; k++) H.cc[3 * (size_t)H.map[c] + k] += centres[3 * (size_t)c + k];
-                cn[H.map[c]]++;
-            }
-            for (int C = 0; C < nCoarse; C++)
-                for (int k = 0; k < 3; k++) H.cc[3 * (size_t)C + k] /= cn[C];
-        }
-        // processor / cyclic interfaces of the coarse level (processorGAMGInterface.C:60-140,
-        // cyclicGAMGInterface.C:70-150): unique
-        // (master cell, slave cell) pairs in order of first appearance along every fine patch
-        H.nFinePF = nPatches ? fPatchStart[nPatches] : 0;
-        H.pfRestrict.assign(std::max(H.nFinePF, 1), 0);
-        H.cPatchStart.assign((size_t)nPatches + 1, 0);
-        if (nPatches) {
-            std::vector<int> sendMap(H.nFinePF), nbrMap(H.nFinePF);
-            for (int i = 0; i < H.nFinePF; i++) sendMap[i] = H.map[fFaceCells[i]];
-            rc = comm_exchange_patch_ints(a->ctx, nPatches, fPatchStart.data(), a->neighbRank.data(), sendMap.data(),
-                                          nbrMap.data());
-            if (rc != B200LDU_OK) break;
-            int nC = 0;
-            for (int p = 0; p < nPatches; p++) {
-                const int nb = a->neighbRank[p], me = a->ctx->rank;
-                // master side first so that both sides enumerate the same pairs: the lower rank of a processor
-                // patch, the owner (= lower patch index) of a cyclic pair (cyclicGAMGInterface.C:104-127)
-                const bool master = nb >= 0 ? (me < nb) : (p < -nb - 1);
-                H.cPatchStart[p] = nC;
-                std::vector<std::pair<int, int>> pairs;
-                for (int i = fPatchStart[p]; i < fPatchStart[p + 1]; i++) {
-                    std::pair<int, int> pr = master ? std::make_pair(sendMap[i], nbrMap[i])
-                                                    : std::make_pair(nbrMap[i], sendMap[i]);
-                    int found = -1;
-                    for (int k = (int)pairs.size() - 1; k >= 0; k--)
-                        if (pairs[k] == pr) {
-                            found = k;
-                            break;
-                        }
-                    if (found < 0) {
-                        found = (int)pairs.size();
-                        pairs.push_back(pr);
-                        H.cFaceCells.push_back(sendMap[i]);
-                    }
-                    H.pfRestrict[i] = nC + found;
-                }
-                nC += (int)pairs.size();
-            }
-            H.cPatchStart[nPatches] = nC;
-            H.nCoarsePF = nC;
-        }
-        // restrictFaceField of the weights for the next step (pairGAMGAgglomerate.C:86-107)
-        std::vector<double> cw(H.nCoarseFaces, 0.0);
-        for (int f = 0; f < H.nFineFaces; f++)
-            if (H.faceRestrict[f] >= 0) cw[H.faceRestrict[f]] += w[f];
-        w.swap(cw);
-        lo = H.cOwner;
-        up = H.cNeigh;
-        fPatchStart = H.cPatchStart;
-        fFaceCells = H.cFaceCells;
-        centres = H.cc;
-        nFine = nCoarse;
-        if (nPairLevels % mergeLevels) { // pairGAMGAgglomerate.C:110-117
-            combine(pend, H);
-        } else {
-            if (havePend) {
-                rc = finalize(pend);
-                if (rc != B200LDU_OK) break;
-            }
-            pend = std::move(H);
-            havePend = true;
-        }
-        nPairLevels++;
-    }
-    if (rc == B200LDU_OK && havePend) rc = finalize(pend);
-    if (forwardInOut) *forwardInOut = forward ? 1 : 0;
+    if (rc == B200LDU_OK && !H.empty() && !a->hostOnly) rc = coarsest_setup(g, a, H.back());
+    for (size_t k = 0; k < H.size() && rc == B200LDU_OK; k++)
+        rc = level_upload(g, k ? g->lev[k - 1].addr : a, std::move(H[k]));
     if (rc != B200LDU_OK) {
         b200ldu_gamg_destroy(g);
         return rc;
     }
     g->nLevels = (int)g->lev.size();
-    // coarsest level across the ranks: sizes, offsets and the neighbour-side cell of every
-    // coarsest processor-patch face (columns of the global matrix, LUscalarMatrix.C:201-270)
-    if (g->nLevels > 0 && (a->ctx->nRanks > 1 || nPatches)) {
-        GamgLevel &LC = g->lev[g->nLevels - 1];
-        const int R = a->ctx->nRanks;
-        double mine = LC.nCoarse;
-        std::vector<double> all(R);
-        rc = comm_allgather_host(a->ctx, &mine, 1, all.data());
-        if (rc == B200LDU_OK) {
-            g->coarsestCounts.resize(R);
-            g->coarsestOffs.assign(R + 1, 0);
-            g->nMaxCoarsest = 0;
-            for (int r = 0; r < R; r++) {
-                g->coarsestCounts[r] = (int)all[r];
-                g->coarsestOffs[r + 1] = g->coarsestOffs[r] + g->coarsestCounts[r];
-                g->nMaxCoarsest = std::max(g->nMaxCoarsest, g->coarsestCounts[r]);
-            }
-            if (R > 1 && g->nMaxCoarsest > P2P_GMAX) {
-                b200_set_error("GAMG: coarsest level has %d cells on one rank; the multi-rank direct solve "
-                               "supports up to %d (lower nCellsInCoarsestLevel)", g->nMaxCoarsest, P2P_GMAX);
-                rc = B200LDU_EINVAL;
-            }
-        }
-        if (rc == B200LDU_OK && nPatches) {
-            g->coarsestNbrCell.resize(std::max(LC.nCoarsePF, 1));
-            rc = comm_exchange_patch_ints(a->ctx, nPatches, LC.cPatchStart.data(), a->neighbRank.data(),
-                                          LC.cFaceCells.data(), g->coarsestNbrCell.data());
-        }
-        if (rc != B200LDU_OK) {
-            b200ldu_gamg_destroy(g);
-            return rc;
-        }
-    }
     *out = g;
     return B200LDU_OK;
 }
@@ -684,22 +686,19 @@ __global__ void dense_apply_kernel(int n, const double *__restrict__ inv, const 
     }
 }
 
-#define LAUNCH1D(kernel, n, st, ...)                                      \
-    do {                                                                  \
-        if ((n) > 0) {                                                    \
-            kernel<<<((n) + 255) / 256, 256, 0, st>>>(__VA_ARGS__);       \
-            S.ctx->launches++;                                            \
-        }                                                                 \
-    } while (0)
-
 // ---------------------------------------------------------------------------
 // solve
 // ---------------------------------------------------------------------------
 namespace {
 
-struct LevelView { // uniform access to the finest matrix (-1) and coarse level k
-    b200ldu_matrix *m;
-};
+// kernel(n, args...) with one thread per item, 256 per CTA, on the solve's stream; n <= 0 launches nothing
+template <class... P, class... A>
+void launch1d(Solve &S, void (*kernel)(int, P...), int n, A... args)
+{
+    if (n <= 0) return;
+    kernel<<<(n + 255) / 256, 256, 0, S.ctx->stream>>>(n, args...);
+    S.ctx->launches++;
+}
 
 int smooth_in_place(Solve &S, b200ldu_matrix *m, double omega, double *&x, double *&spare, const double *b,
                     int nSweeps, const int *stop)
@@ -738,7 +737,6 @@ int gamg_scale(Solve &S, b200ldu_matrix *m, double *field, double *Acf, const do
 static int gamg_build_matrices(Solve &S, b200ldu_gamg *g)
 {
     b200ldu_matrix *fm = S.m;
-    cudaStream_t st = S.ctx->stream;
     const double *fd = fm->diag_ext, *fu = fm->upper_ext, *fl = fm->symmetric ? nullptr : fm->lower_ext;
     const double *fb = fm->bou_ext, *fi = fm->int_ext;
     if (!fd || !fu) {
@@ -747,14 +745,10 @@ static int gamg_build_matrices(Solve &S, b200ldu_gamg *g)
     }
     for (int k = 0; k < g->nLevels; k++) {
         GamgLevel &L = g->lev[k];
-        LAUNCH1D(agg_diag_kernel, L.nCoarse, st, L.nCoarse, L.d_cellChildStart, L.d_cellChild, L.d_diagFaceStart,
-                 L.d_diagFace, fd, fu, fl, L.d_diag);
-        LAUNCH1D(agg_faces_kernel, L.nCoarseFaces, st, L.nCoarseFaces, L.d_faceChildStart, L.d_faceChild, fu, fl,
-                 L.d_upper, L.d_lower);
-        if (L.nCoarsePF > 0) {
-            LAUNCH1D(agg_patch_kernel, L.nCoarsePF, st, L.nCoarsePF, L.d_pfChildStart, L.d_pfChild, fb, fi, L.d_bou,
-                     L.d_int);
-        }
+        launch1d(S, agg_diag_kernel, L.nCoarse, L.d_cellChildStart, L.d_cellChild, L.d_diagFaceStart, L.d_diagFace, fd,
+                 fu, fl, L.d_diag);
+        launch1d(S, agg_faces_kernel, L.nCoarseFaces, L.d_faceChildStart, L.d_faceChild, fu, fl, L.d_upper, L.d_lower);
+        launch1d(S, agg_patch_kernel, L.nCoarsePF, L.d_pfChildStart, L.d_pfChild, fb, fi, L.d_bou, L.d_int);
         KERNEL_CHECK();
         // identical boundary/internal interface coefficients on the finest level stay identical
         const double *cInt = (fm->bou_ext == fm->int_ext) ? L.d_bou : L.d_int;
@@ -878,26 +872,11 @@ static int gamg_coarsest_inverse(Solve &S, b200ldu_gamg *g)
     return B200LDU_OK;
 }
 
-template <class Body>
-int run_iterations(Solve &S, long long maxBodies, Body body); // solvers.cu
-int init_residual(Solve &S, const double *psi, const double *b, const double *wA, double *rA, double *tmp,
-                  const double *wT, double *rT); // solvers.cu
-int gamg_run_cycles(Solve &S, long long maxBodies, int (*body)(void *), void *arg); // solvers.cu
-
-struct CycleArgs {
-    Solve *S;
-    b200ldu_gamg *g;
-    int scaleCorrection;
-    double *psiBuf[2];
-    long long finestSweeps;
-    double *Apsi, *finestCorr, *finestRes;
-};
-
-static int gamg_cycle(void *vp)
+// One V-cycle and the finest residual.  psi ping-pongs between psiBuf[0] and [1] with the finest sweeps, counted on
+// the host in finestSweeps; the interpolated correction swaps finestCorr and Apsi.
+static int gamg_cycle(Solve &S, b200ldu_gamg *g, int scaleCorrection, double *const psiBuf[2], long long &finestSweeps,
+                      double *&Apsi, double *&finestCorr, double *finestRes)
 {
-    CycleArgs &A = *(CycleArgs *)vp;
-    Solve &S = *A.S;
-    b200ldu_gamg *g = A.g;
     const b200ldu_controls &c = S.c;
     SolverScalars *sc = S.sc;
     double *hist = S.hist;
@@ -911,7 +890,7 @@ static int gamg_cycle(void *vp)
     // ---- Vcycle (GAMGSolverSolve.C:181-474) ----
     {
         GamgLevel &L0 = g->lev[0];
-        LAUNCH1D(restrict_kernel, L0.nCoarse, st, L0.nCoarse, L0.d_childStart, L0.d_child, A.finestRes, L0.src, stop);
+        launch1d(S, restrict_kernel, L0.nCoarse, L0.d_childStart, L0.d_child, finestRes, L0.src, stop);
     }
     for (int k = 0; k < coarsest; k++) {
         GamgLevel &L = g->lev[k], &Ln = g->lev[k + 1];
@@ -919,7 +898,7 @@ static int gamg_cycle(void *vp)
             CUDA_TRY(cudaMemsetAsync(L.corr, 0, sizeof(double) * (size_t)L.addr->vecLen, st));
             TRY(smooth_in_place(S, L.mat, omega, L.corr, L.tmp, L.src,
                                 imin(c.nPreSweeps + c.preSweepsLevelMultiplier * k, c.maxPreSweeps), stop));
-            if (A.scaleCorrection && k < coarsest - 1) TRY(gamg_scale(S, L.mat, L.corr, L.acf, L.src, stop));
+            if (scaleCorrection && k < coarsest - 1) TRY(gamg_scale(S, L.mat, L.corr, L.acf, L.src, stop));
             TRY(mat_amul(L.mat, false, L.corr, L.acf, 0, nullptr, nullptr, stop));
             double *src = L.src, *acf = L.acf;
             TRY(ew_launch<0>(S.ctx, L.addr->L.nPad / 2, stop, nullptr, nullptr, [=] __device__(int i, double *) {
@@ -927,7 +906,7 @@ static int gamg_cycle(void *vp)
                 V2(src)[i] = make_double2(__dsub_rn(s2.x, a2.x), __dsub_rn(s2.y, a2.y));
             }));
         }
-        LAUNCH1D(restrict_kernel, Ln.nCoarse, st, Ln.nCoarse, Ln.d_childStart, Ln.d_child, L.src, Ln.src, stop);
+        launch1d(S, restrict_kernel, Ln.nCoarse, Ln.d_childStart, Ln.d_child, L.src, Ln.src, stop);
     }
     { // solveCoarsestLevel :552-619
         GamgLevel &L = g->lev[coarsest];
@@ -994,12 +973,12 @@ static int gamg_cycle(void *vp)
         int nPadL = L.addr->L.nPad;
         if (c.nPreSweeps)
             CUDA_TRY(cudaMemcpyAsync(L.pre, L.corr, sizeof(double) * (size_t)L.addr->vecLen, cudaMemcpyDeviceToDevice, st));
-        LAUNCH1D(prolong_kernel, nPadL, st, nPadL, Ln.d_pmap, Ln.corr, L.corr, stop);
+        launch1d(S, prolong_kernel, nPadL, Ln.d_pmap, Ln.corr, L.corr, stop);
         if (c.interpolateCorrection) {
             TRY(mat_interpolate(L.mat, L.corr, L.tmp, stop));
             std::swap(L.corr, L.tmp);
         }
-        if (A.scaleCorrection && (c.interpolateCorrection || k < coarsest - 1))
+        if (scaleCorrection && (c.interpolateCorrection || k < coarsest - 1))
             TRY(gamg_scale(S, L.mat, L.corr, L.acf, L.src, stop));
         if (c.nPreSweeps) {
             double *corr = L.corr, *pre = L.pre;
@@ -1013,34 +992,31 @@ static int gamg_cycle(void *vp)
     }
     {
         GamgLevel &L0 = g->lev[0];
-        int nPadF = fm->a->L.nPad;
-        LAUNCH1D(prolong_kernel, nPadF, st, nPadF, L0.d_pmap, L0.corr, A.finestCorr, stop);
+        launch1d(S, prolong_kernel, fm->a->L.nPad, L0.d_pmap, L0.corr, finestCorr, stop);
         KERNEL_CHECK();
     }
-    double *psi = A.psiBuf[A.finestSweeps & 1], *spare = A.psiBuf[(A.finestSweeps + 1) & 1];
+    double *psi = psiBuf[finestSweeps & 1], *spare = psiBuf[(finestSweeps + 1) & 1];
     if (c.interpolateCorrection) {
-        TRY(mat_interpolate(fm, A.finestCorr, A.Apsi, stop));
-        std::swap(A.finestCorr, A.Apsi);
+        TRY(mat_interpolate(fm, finestCorr, Apsi, stop));
+        std::swap(finestCorr, Apsi);
     }
-    if (A.scaleCorrection) TRY(gamg_scale(S, fm, A.finestCorr, A.Apsi, A.finestRes, stop));
+    if (scaleCorrection) TRY(gamg_scale(S, fm, finestCorr, Apsi, finestRes, stop));
     {
-        double *fc = A.finestCorr;
+        double *fc = finestCorr;
         TRY(ew_launch<0>(S.ctx, fm->a->L.nPad / 2, stop, nullptr, nullptr, [=] __device__(int i, double *) {
             double2 p2 = CV2(psi)[i], c2 = CV2(fc)[i];
             V2(psi)[i] = make_double2(__dadd_rn(p2.x, c2.x), __dadd_rn(p2.y, c2.y));
         }));
     }
-    for (int s = 0; s < c.nFinestSweeps; s++) {
-        TRY(mat_jacobi(fm, omega, psi, S.src, spare, stop));
-        std::swap(psi, spare);
-        A.finestSweeps++;
-    }
+    const int nFinest = c.nFinestSweeps > 0 ? c.nFinestSweeps : 0;
+    TRY(smooth_in_place(S, fm, omega, psi, spare, S.src, nFinest, stop));
+    finestSweeps += nFinest;
     // ---- finest residual + convergence (:146-175) ----
-    TRY(mat_amul(fm, false, psi, A.Apsi, 0, nullptr, nullptr, stop));
+    TRY(mat_amul(fm, false, psi, Apsi, 0, nullptr, nullptr, stop));
     int np = 0;
     {
-        const double *b = S.src, *Ap = A.Apsi;
-        double *fr = A.finestRes;
+        const double *b = S.src, *Ap = Apsi;
+        double *fr = finestRes;
         TRY(ew_launch<1>(S.ctx, fm->a->L.nPad / 2, stop, S.partials, &np, [=] __device__(int i, double *red) {
             double2 b2 = CV2(b)[i], a2 = CV2(Ap)[i];
             double2 r = make_double2(__dsub_rn(b2.x, a2.x), __dsub_rn(b2.y, a2.y));
@@ -1072,17 +1048,10 @@ int gamg_solve(Solve &S, b200ldu_gamg *g, const char *smoother)
         return B200LDU_EINVAL;
     }
     b200ldu_matrix *fm = S.m;
-    CycleArgs A;
-    A.S = &S;
-    A.g = g;
-    A.scaleCorrection = S.c.scaleCorrection < 0 ? (fm->symmetric ? 1 : 0) : S.c.scaleCorrection;
-    A.psiBuf[0] = S.psi;
-    A.psiBuf[1] = S.vec(0);
-    A.Apsi = S.vec(1);
-    A.finestCorr = S.vec(2);
-    A.finestRes = S.vec(3);
-    A.finestSweeps = 0;
-    if (!A.psiBuf[1] || !A.Apsi || !A.finestCorr || !A.finestRes) return B200LDU_ECUDA;
+    const int scaleCorrection = S.c.scaleCorrection < 0 ? (fm->symmetric ? 1 : 0) : S.c.scaleCorrection;
+    double *const psiBuf[2] = {S.psi, S.vec(0)};
+    double *Apsi = S.vec(1), *finestCorr = S.vec(2), *finestRes = S.vec(3);
+    if (!psiBuf[1] || !Apsi || !finestCorr || !finestRes) return B200LDU_ECUDA;
 
     TRY(gamg_build_matrices(S, g));
     if (S.c.directSolveCoarsest) {
@@ -1091,14 +1060,18 @@ int gamg_solve(Solve &S, b200ldu_gamg *g, const char *smoother)
         S.useGraph = false; // the coarsest-level Krylov solve synchronises with the host
         S.c.checkEvery = 1;
     }
-    TRY(mat_amul(fm, false, S.psi, A.Apsi, 0, nullptr, nullptr, nullptr));
-    TRY(init_residual(S, S.psi, S.src, A.Apsi, A.finestRes, A.finestCorr, nullptr, nullptr));
+    TRY(mat_amul(fm, false, S.psi, Apsi, 0, nullptr, nullptr, nullptr));
+    TRY(init_residual(S, S.psi, S.src, Apsi, finestRes, finestCorr));
     long long maxBodies = S.c.maxIter > S.c.minIter ? S.c.maxIter : S.c.minIter;
     if (maxBodies < 1) maxBodies = 1;
-    TRY(gamg_run_cycles(S, maxBodies, gamg_cycle, &A));
-    S.sweepParityUnknown = S.c.nFinestSweeps > 0;
-    S.smoothBuf[0] = A.psiBuf[0];
-    S.smoothBuf[1] = A.psiBuf[1];
-    S.gamgFinestSweeps = S.c.nFinestSweeps;
+    // counted when a cycle is enqueued, so not on graph replays: a captured chunk has an even number of cycles, which
+    // brings the parity back to the buffers the capture started from
+    long long finestSweeps = 0;
+    TRY(run_iterations(S, maxBodies, [&](long long) {
+        return gamg_cycle(S, g, scaleCorrection, psiBuf, finestSweeps, Apsi, finestCorr, finestRes);
+    }));
+    S.smoothBuf[0] = psiBuf[0];
+    S.smoothBuf[1] = psiBuf[1];
+    S.sweepsPerIteration = S.c.nFinestSweeps > 0 ? S.c.nFinestSweeps : 0;
     return B200LDU_OK;
 }

@@ -255,3 +255,23 @@ int dev_upload(T **d, const std::vector<T> &h)
     if (h.size()) CUDA_TRY(cudaMemcpy(*d, h.data(), sizeof(T) * h.size(), cudaMemcpyHostToDevice));
     return B200LDU_OK;
 }
+
+// device array of n (at least one) T, recorded in mem, whose owner frees every pointer in it
+template <class T>
+int dev_alloc(std::vector<void *> &mem, T *&d, size_t n)
+{
+    CUDA_TRY(cudaMalloc((void **)&d, sizeof(T) * (n ? n : 1)));
+    mem.push_back(d);
+    return B200LDU_OK;
+}
+
+// uploads h into a new device array recorded in mem
+template <class Ptr, class T>
+int upload(std::vector<void *> &mem, Ptr &d, const std::vector<T> &h)
+{
+    T *p = nullptr;
+    TRY(dev_alloc(mem, p, h.size()));
+    d = p;
+    if (h.size()) CUDA_TRY(cudaMemcpy(p, h.data(), sizeof(T) * h.size(), cudaMemcpyHostToDevice));
+    return B200LDU_OK;
+}

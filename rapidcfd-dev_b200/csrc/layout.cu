@@ -547,42 +547,33 @@ void fill_face_stream(const Graph &g, const std::vector<int> &perm, Plan &P)
     }
 }
 
-// uploads h and records the allocation in a->layoutMem, which b200ldu_addr_destroy frees
-template <class Ptr, class T>
-int upload(b200ldu_addr *a, Ptr &d, const std::vector<T> &h)
-{
-    T *p = nullptr;
-    const int rc = dev_upload(&p, h);
-    if (p) a->layoutMem.push_back(p);
-    d = p;
-    return rc;
-}
-
-// ---- 8. device path: upload the record, set every layout field of the addressing ----
+// ---- 8. device path: upload the record (into a->layoutMem, which b200ldu_addr_destroy frees), set every layout
+// field of the addressing ----
 int layout_upload(b200ldu_addr *a, const Graph &g, const LayoutHost &H)
 {
     LayoutDev &L = a->L;
-    TRY(upload(a, L.sliceStart, H.sliceStart));
-    TRY(upload(a, L.sliceW, H.sliceW));
-    TRY(upload(a, L.sliceWL, H.sliceWL));
-    TRY(upload(a, L.col, H.col));
-    TRY(upload(a, a->d_code, H.code));
-    TRY(upload(a, L.haloStart, H.haloStart));
-    TRY(upload(a, L.haloIdx, H.haloIdx));
-    TRY(upload(a, L.perm, a->perm_h));
-    TRY(upload(a, L.iperm, a->iperm_h));
-    TRY(upload(a, L.sendRows, H.sendRows));
-    TRY(upload(a, a->d_l, a->l));
-    TRY(upload(a, a->d_u, a->u));
-    TRY(upload(a, a->d_ownerStart, g.ownerStart));
-    TRY(upload(a, a->d_losort, g.losort));
-    TRY(upload(a, a->d_losortStart, g.losortStart));
+    std::vector<void *> &mem = a->layoutMem;
+    TRY(upload(mem, L.sliceStart, H.sliceStart));
+    TRY(upload(mem, L.sliceW, H.sliceW));
+    TRY(upload(mem, L.sliceWL, H.sliceWL));
+    TRY(upload(mem, L.col, H.col));
+    TRY(upload(mem, a->d_code, H.code));
+    TRY(upload(mem, L.haloStart, H.haloStart));
+    TRY(upload(mem, L.haloIdx, H.haloIdx));
+    TRY(upload(mem, L.perm, a->perm_h));
+    TRY(upload(mem, L.iperm, a->iperm_h));
+    TRY(upload(mem, L.sendRows, H.sendRows));
+    TRY(upload(mem, a->d_l, a->l));
+    TRY(upload(mem, a->d_u, a->u));
+    TRY(upload(mem, a->d_ownerStart, g.ownerStart));
+    TRY(upload(mem, a->d_losort, g.losort));
+    TRY(upload(mem, a->d_losortStart, g.losortStart));
     if (H.hasFs) {
-        TRY(upload(a, L.fsSlice, H.fsSlice));
-        TRY(upload(a, L.fsCT, H.fsCT));
-        TRY(upload(a, a->d_fsCode, H.fsCode));
-        TRY(upload(a, L.fsListStart, H.fsListStart));
-        TRY(upload(a, L.fsListIfc, H.fsListIfc));
+        TRY(upload(mem, L.fsSlice, H.fsSlice));
+        TRY(upload(mem, L.fsCT, H.fsCT));
+        TRY(upload(mem, a->d_fsCode, H.fsCode));
+        TRY(upload(mem, L.fsListStart, H.fsListStart));
+        TRY(upload(mem, L.fsListIfc, H.fsListIfc));
     }
     L.nCells = g.nCells;
     L.nPad = H.nPad;

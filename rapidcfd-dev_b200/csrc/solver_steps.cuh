@@ -1,4 +1,4 @@
-// solver_steps.cuh -- device-side scalar logic shared by solvers.cu and gamg.cu
+// solver_steps.cuh -- device-side scalar logic and the host iteration driver, shared by solvers.cu and gamg.cu
 #pragma once
 #include "comm.h"
 #include "ops.cuh"
@@ -64,4 +64,80 @@ template <int NRED, class G>
 int scalar_step(Solve &S, int nPartials, G g)
 {
     return scalar_step_on<NRED>(S, S.partials, nPartials, g);
+}
+
+// ---------------------------------------------------------------------------
+// host driver: enqueue iteration bodies, poll the device stop flag (pipelined)
+// ---------------------------------------------------------------------------
+template <class Body>
+int run_iterations(Solve &S, long long maxBodies, Body body)
+{
+    b200ldu_ctx *ctx = S.ctx;
+    int every = S.c.checkEvery > 0 ? S.c.checkEvery : 8;
+    volatile int *flags = (volatile int *)S.pinnedFlags; // two slots
+    cudaEvent_t ev[2] = {S.ev[0], S.ev[1]};
+    long long enq = 0;
+    int chunk = 0;
+    bool pending[2] = {false, false};
+    cudaGraphExec_t graphExec = nullptr;
+    long long launchesPerGraph = 0;
+    struct GraphGuard {
+        cudaGraphExec_t &g;
+        ~GraphGuard()
+        {
+            if (g) cudaGraphExecDestroy(g);
+        }
+    } guard{graphExec};
+    for (;;) {
+        int slot = chunk & 1;
+        // before reusing a slot, consume its previous result
+        if (pending[slot]) {
+            CUDA_TRY(cudaEventSynchronize(ev[slot]));
+            pending[slot] = false;
+            if (flags[slot]) break;
+        }
+        if (enq >= maxBodies) {
+            // nothing more to enqueue: drain the other slot and leave
+            int o = slot ^ 1;
+            if (pending[o]) {
+                CUDA_TRY(cudaEventSynchronize(ev[o]));
+                pending[o] = false;
+            }
+            break;
+        }
+        // CUDA graph: after one chunk launched kernel by kernel (attribute set-up, warm caches) a full
+        // chunk of `every` bodies (even, so every ping-pong returns to its starting buffers) is captured
+        // once and replayed -- the device-side stop flag makes replayed bodies after convergence no-ops.
+        const bool fullChunk = (enq + every <= maxBodies) && (every % 2 == 0) && (enq % 2 == 0);
+        if (S.useGraph && fullChunk && chunk >= 1) {
+            if (!graphExec) {
+                long long l0 = ctx->launches;
+                cudaGraph_t g = nullptr;
+                CUDA_TRY(cudaStreamBeginCapture(ctx->stream, cudaStreamCaptureModeRelaxed));
+                int rcb = B200LDU_OK;
+                for (int k = 0; k < every && rcb == B200LDU_OK; k++) rcb = body(enq + k);
+                cudaError_t ce = cudaStreamEndCapture(ctx->stream, &g);
+                if (rcb != B200LDU_OK) return rcb;
+                if (ce != cudaSuccess || !g) {
+                    b200_set_error("CUDA graph capture failed: %s", cudaGetErrorString(ce));
+                    return B200LDU_ECUDA;
+                }
+                launchesPerGraph = ctx->launches - l0;
+                ctx->launches = l0;
+                CUDA_TRY(cudaGraphInstantiate(&graphExec, g, 0));
+                cudaGraphDestroy(g);
+            }
+            CUDA_TRY(cudaGraphLaunch(graphExec, ctx->stream));
+            ctx->launches += launchesPerGraph;
+            enq += every;
+        } else {
+            for (int k = 0; k < every && enq < maxBodies; k++, enq++) TRY(body(enq));
+        }
+        CUDA_TRY(cudaMemcpyAsync((void *)&flags[slot], &S.sc->stop, sizeof(int), cudaMemcpyDeviceToHost,
+                                 ctx->stream));
+        CUDA_TRY(cudaEventRecord(ev[slot], ctx->stream));
+        pending[slot] = true;
+        chunk++;
+    }
+    return B200LDU_OK;
 }

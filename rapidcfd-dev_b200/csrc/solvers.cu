@@ -20,7 +20,7 @@
 // initial residual, normFactor and the first convergence test, common to all solvers
 // (PCG.C:92-128; lduMatrixSolver.C:205-236).  wA must hold A.psi; tmp receives sumA.
 int init_residual(Solve &S, const double *psi, const double *b, const double *wA, double *rA, double *tmp,
-                  const double *wT = nullptr, double *rT = nullptr)
+                  const double *wT, double *rT)
 {
     b200ldu_addr *a = S.m->a;
     SolverScalars *sc = S.sc;
@@ -59,82 +59,6 @@ int init_residual(Solve &S, const double *psi, const double *b, const double *wA
         bool conv = check_convergence(s);
         if (!(s->minIter > 0 || !conv)) s->stop = 1;
     }));
-    return B200LDU_OK;
-}
-
-// ---------------------------------------------------------------------------
-// host driver: enqueue iteration bodies, poll the device stop flag (pipelined)
-// ---------------------------------------------------------------------------
-template <class Body>
-int run_iterations(Solve &S, long long maxBodies, Body body)
-{
-    b200ldu_ctx *ctx = S.ctx;
-    int every = S.c.checkEvery > 0 ? S.c.checkEvery : 8;
-    volatile int *flags = (volatile int *)S.pinnedFlags; // two slots
-    cudaEvent_t ev[2] = {S.ev[0], S.ev[1]};
-    long long enq = 0;
-    int chunk = 0;
-    bool pending[2] = {false, false};
-    cudaGraphExec_t graphExec = nullptr;
-    long long launchesPerGraph = 0;
-    struct GraphGuard {
-        cudaGraphExec_t &g;
-        ~GraphGuard()
-        {
-            if (g) cudaGraphExecDestroy(g);
-        }
-    } guard{graphExec};
-    for (;;) {
-        int slot = chunk & 1;
-        // before reusing a slot, consume its previous result
-        if (pending[slot]) {
-            CUDA_TRY(cudaEventSynchronize(ev[slot]));
-            pending[slot] = false;
-            if (flags[slot]) break;
-        }
-        if (enq >= maxBodies) {
-            // nothing more to enqueue: drain the other slot and leave
-            int o = slot ^ 1;
-            if (pending[o]) {
-                CUDA_TRY(cudaEventSynchronize(ev[o]));
-                pending[o] = false;
-            }
-            break;
-        }
-        // CUDA graph: after one chunk launched kernel by kernel (attribute set-up, warm caches) a full
-        // chunk of `every` bodies (even, so every ping-pong returns to its starting buffers) is captured
-        // once and replayed -- the device-side stop flag makes replayed bodies after convergence no-ops.
-        const bool fullChunk = (enq + every <= maxBodies) && (every % 2 == 0) && (enq % 2 == 0);
-        if (S.useGraph && fullChunk && chunk >= 1) {
-            if (!graphExec) {
-                long long l0 = ctx->launches;
-                cudaGraph_t g = nullptr;
-                CUDA_TRY(cudaStreamBeginCapture(ctx->stream, cudaStreamCaptureModeRelaxed));
-                int rcb = B200LDU_OK;
-                for (int k = 0; k < every && rcb == B200LDU_OK; k++) rcb = body(enq + k);
-                cudaError_t ce = cudaStreamEndCapture(ctx->stream, &g);
-                if (rcb != B200LDU_OK) return rcb;
-                if (ce != cudaSuccess || !g) {
-                    b200_set_error("CUDA graph capture failed: %s", cudaGetErrorString(ce));
-                    return B200LDU_ECUDA;
-                }
-                launchesPerGraph = ctx->launches - l0;
-                ctx->launches = l0;
-                CUDA_TRY(cudaGraphInstantiate(&graphExec, g, 0));
-                cudaGraphDestroy(g);
-            }
-            CUDA_TRY(cudaGraphLaunch(graphExec, ctx->stream));
-            ctx->launches += launchesPerGraph;
-            enq += every;
-        } else {
-            for (int k = 0; k < every && enq < maxBodies; k++, enq++) TRY(body(enq));
-        }
-        CUDA_TRY(cudaMemcpyAsync((void *)&flags[slot], &S.sc->stop, sizeof(int), cudaMemcpyDeviceToHost,
-                                 ctx->stream));
-        CUDA_TRY(cudaEventRecord(ev[slot], ctx->stream));
-        pending[slot] = true;
-        chunk++;
-    }
     return B200LDU_OK;
 }
 
@@ -578,7 +502,7 @@ int solve_smooth(Solve &S)
     int per = nSweeps > 0 ? nSweeps : 1;
     long long maxBodies = ((long long)(S.c.maxIter > S.c.minIter ? S.c.maxIter : S.c.minIter) + per - 1) / per + 1;
     TRY(run_iterations(S, maxBodies, body));
-    S.sweepParityUnknown = true; // resolved from nIterations after the read-back
+    S.sweepsPerIteration = 1; // nIterations counts sweeps; the buffer is picked after the read-back
     S.smoothBuf[0] = buf[0];
     S.smoothBuf[1] = buf[1];
     return B200LDU_OK;
@@ -594,11 +518,6 @@ int solve_diagonal(Solve &S)
         double2 bb = CV2(b)[i], dd = CV2(d)[i];
         V2(psi)[i] = make_double2(__ddiv_rn(bb.x, dd.x), __ddiv_rn(bb.y, dd.y));
     });
-}
-
-int gamg_run_cycles(Solve &S, long long maxBodies, int (*body)(void *), void *arg)
-{
-    return run_iterations(S, maxBodies, [&](long long) -> int { return body(arg); });
 }
 
 double *Solve::vec(int k)
@@ -802,11 +721,7 @@ int solve_banded(b200ldu_matrix *m, const char *solver, const char *pre, const b
             perf->singular = hp->singular;
         }
         if (S.fixedSweeps) perf->nIterations = S.fixedSweeps;
-        if (S.sweepParityUnknown) {
-            long long sweeps = perf->nIterations; // smoothSolver: nIterations counts sweeps
-            if (S.gamgFinestSweeps) sweeps = (long long)perf->nIterations * S.gamgFinestSweeps;
-            S.resultBuf = S.smoothBuf[sweeps & 1];
-        }
+        if (S.sweepsPerIteration) S.resultBuf = S.smoothBuf[((long long)perf->nIterations * S.sweepsPerIteration) & 1];
         if (S.resultBuf) *resultBuf = S.resultBuf;
         if (S.hist && hist_h) {
             int k = perf->nIterations + 1;

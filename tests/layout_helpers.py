@@ -23,9 +23,10 @@ def debug_lib(capi):
     return L
 
 
-def debug_layout(capi, mesh, centres=True, band=None, patches=None):
-    """{name: array} of the layout of `mesh` (its own coupled patches unless `patches` = (patchStart, faceCells)),
-    built with B200LDU_BAND_ROWS=band, or without the variable when band is None."""
+def debug_addr(capi, mesh, centres=True, band=None, patches=None):
+    """Handle of the host-only addressing of `mesh` (its own coupled patches unless `patches` = (patchStart,
+    faceCells)), built with B200LDU_BAND_ROWS=band, or without the variable when band is None.  The caller frees it
+    with b200ldu_layout_debug_destroy."""
     L = debug_lib(capi)
     ps, fc = patches if patches is not None else mesh.patch_start_facecells()
     ps, fc = np.ascontiguousarray(ps, np.int32), np.ascontiguousarray(fc, np.int32)
@@ -46,6 +47,13 @@ def debug_layout(capi, mesh, centres=True, band=None, patches=None):
         if old is not None:
             os.environ["B200LDU_BAND_ROWS"] = old
     assert rc == 0, L.b200ldu_last_error()
+    return h
+
+
+def debug_layout(capi, mesh, centres=True, band=None, patches=None):
+    """{name: array} of the layout of `mesh`, arguments as debug_addr."""
+    L = debug_lib(capi)
+    h = debug_addr(capi, mesh, centres, band, patches)
     out = {}
     for what, (name, dt) in enumerate(WHAT):
         n = L.b200ldu_layout_debug_get(h, what, None, 0)
