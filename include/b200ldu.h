@@ -182,6 +182,10 @@ int b200ldu_solve_host(b200ldu_matrix *m, const char *solver, const char *precon
                        const double *source_h, b200ldu_perf *perf, double *hist_h, int histCap);
 /* number of library kernels launched on this context since creation */
 long long b200ldu_launch_count(const b200ldu_ctx *ctx);
+/* device memory of the handles created on this context (addressings, matrices, GAMG hierarchies): the bytes they
+ * hold now, and the number of device allocations they have made since the context was created.  Either pointer may
+ * be NULL.  Unlike cudaMemGetInfo it counts this library's memory only. */
+int b200ldu_ctx_device_mem(const b200ldu_ctx *ctx, long long *liveBytes, long long *nAllocs);
 
 /* ---- GAMGAgglomeration (pair agglomeration, cached on the mesh:
  * LDU/solvers/GAMG/GAMGAgglomerations/..., GAMGAgglomeration.C:132-233) ----

@@ -57,7 +57,7 @@ EXPORTS = [
     "b200ldu_amul", "b200ldu_tmul", "b200ldu_sumA", "b200ldu_residual", "b200ldu_H", "b200ldu_H1",
     "b200ldu_faceH", "b200ldu_precondition", "b200ldu_smooth",
     "b200ldu_vec_len", "b200ldu_to_banded", "b200ldu_from_banded", "b200ldu_amul_banded",
-    "b200ldu_solve", "b200ldu_solve_host", "b200ldu_launch_count", "b200ldu_bench_op",
+    "b200ldu_solve", "b200ldu_solve_host", "b200ldu_launch_count", "b200ldu_ctx_device_mem", "b200ldu_bench_op",
     "b200ldu_gamg_create", "b200ldu_gamg_destroy", "b200ldu_gamg_nlevels", "b200ldu_gamg_level_size",
     "b200ldu_gamg_restrict_addr",
     "b200ldu_fv_boundary_set", "b200ldu_fv_surface_integrate", "b200ldu_fv_gauss_grad",
@@ -91,6 +91,7 @@ def lib():
     L.b200ldu_vec_len.argtypes = [vp]
     L.b200ldu_launch_count.restype = C.c_longlong
     L.b200ldu_launch_count.argtypes = [vp]
+    L.b200ldu_ctx_device_mem.argtypes = [vp, C.POINTER(C.c_longlong), C.POINTER(C.c_longlong)]
     L.b200ldu_controls_default.argtypes = [C.POINTER(Controls)]
     L.b200ldu_ctx_create.argtypes = [C.c_int, C.POINTER(vp)]
     L.b200ldu_ctx_destroy.argtypes = [vp]

@@ -253,21 +253,12 @@ int comm_addr_setup(b200ldu_addr *a)
             pc.push_back({p, a->patchStart[p] + c * PACK_CHUNK, std::min(a->patchStart[p] + (c + 1) * PACK_CHUNK, a->patchStart[p + 1])});
         a->L.nbr[a->L.nNbr++] = nb;
     }
-    PackPatch *d_pp = nullptr;
-    PackChunk *d_pc = nullptr;
-    CUDA_TRY(cudaMalloc((void **)&d_pp, sizeof(PackPatch) * pp.size()));
-    CUDA_TRY(cudaMalloc((void **)&d_pc, sizeof(PackChunk) * pc.size()));
-    CUDA_TRY(cudaMemcpy(d_pp, pp.data(), sizeof(PackPatch) * pp.size(), cudaMemcpyHostToDevice));
-    CUDA_TRY(cudaMemcpy(d_pc, pc.data(), sizeof(PackChunk) * pc.size(), cudaMemcpyHostToDevice));
-    a->d_packPatches = d_pp;
-    a->d_packChunks = d_pc;
-    a->nPackChunks = (int)pc.size();
+    TRY(a->mem.upload(a->L.packPatches, pp));
+    TRY(a->mem.upload(a->L.packChunks, pc));
     a->L.haloFlags = (const unsigned long long *)(ctx->region + P2P_HALOFLAG_OFF);
     a->L.haloSeq = ctx->d_seq + 1;
     a->L.tail0 = (const double *)(ctx->region + P2P_RECV_OFF);
     a->L.tail1 = a->L.tail0 + P2P_RECV_CAP;
-    a->L.packChunks = d_pc;
-    a->L.packPatches = d_pp;
     a->L.seqs = ctx->d_seq;
     a->L.nPackChunks = (int)pc.size();
     a->p2pHalo = true;

@@ -39,14 +39,13 @@ extern "C" int b200ldu_fv_boundary_set(b200ldu_addr *a, int nBFaces, const int *
         for (int i = 0; i < nBFaces; i++) faces[cur[bFaceCells_h[i]]++] = i;
     }
     std::vector<int> fc(bFaceCells_h, bFaceCells_h + nBFaces);
-    for (int **p : {&a->d_bFaceCells, &a->d_bCellStart, &a->d_bCellFaces})
-        if (*p) {
-            cudaFree(*p);
-            *p = nullptr;
-        }
-    TRY(dev_upload(&a->d_bFaceCells, fc));
-    TRY(dev_upload(&a->d_bCellStart, start));
-    TRY(dev_upload(&a->d_bCellFaces, faces));
+    // the lists are rewritten in place: work still queued may read the old ones, and until all three are written the
+    // addressing has no boundary list (an upload that fails leaves it so)
+    CUDA_TRY(cudaStreamSynchronize(a->ctx->stream));
+    a->nBFaces = 0;
+    TRY(a->mem.upload(ADDR_BFACE_CELLS, a->d_bFaceCells, fc));
+    TRY(a->mem.upload(ADDR_BCELL_START, a->d_bCellStart, start));
+    TRY(a->mem.upload(ADDR_BCELL_FACES, a->d_bCellFaces, faces));
     a->nBFaces = nBFaces;
     return B200LDU_OK;
 }

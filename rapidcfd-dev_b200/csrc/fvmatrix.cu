@@ -15,8 +15,6 @@
 // element-wise field algebra around it (the /V, the +source, the max / divide / subtract of relax) is fused
 // into the same pass.  Products are rounded separately and summed in the reference's order, so the results
 // are bit-comparable with the oracle.
-#include <algorithm>
-
 #include "comm.h"
 #include "fieldops_kernels.cuh"
 #include "fvmatrix_kernels.cuh"
@@ -37,9 +35,9 @@ int coupled_lists(b200ldu_addr *a)
     for (int c = 0; c < a->nCells; c++) start[c + 1] += start[c];
     std::vector<int> cur(start.begin(), start.end() - 1);
     for (int i = 0; i < tot; i++) faces[cur[a->faceCells[i]]++] = i;
-    TRY(dev_upload(&a->d_cCellStart, start));
-    TRY(dev_upload(&a->d_cCellFaces, faces));
-    TRY(dev_upload(&a->d_cFaceCells, a->faceCells));
+    TRY(a->mem.upload(a->d_cCellStart, start));
+    TRY(a->mem.upload(a->d_cCellFaces, faces));
+    TRY(a->mem.upload(a->d_cFaceCells, a->faceCells));
     a->nCFaces = tot;
     return B200LDU_OK;
 }
@@ -51,18 +49,6 @@ int lists(b200ldu_addr *a, BoundaryLists *L)
     L->bFaces = a->d_bCellFaces;
     L->cStart = a->nCFaces ? a->d_cCellStart : nullptr;
     L->cFaces = a->d_cCellFaces;
-    return B200LDU_OK;
-}
-
-int scratch(b200ldu_addr *a, int slot, size_t doubles, double **out)
-{
-    if (a->fvmScratchLen[slot] < doubles) {
-        if (a->d_fvmScratch[slot]) CUDA_TRY(cudaFree(a->d_fvmScratch[slot]));
-        a->d_fvmScratch[slot] = nullptr;
-        CUDA_TRY(cudaMalloc((void **)&a->d_fvmScratch[slot], sizeof(double) * std::max<size_t>(doubles, 1)));
-        a->fvmScratchLen[slot] = doubles;
-    }
-    *out = a->d_fvmScratch[slot];
     return B200LDU_OK;
 }
 
@@ -90,7 +76,7 @@ extern "C" int b200ldu_fv_patch_neighbour_field(b200ldu_addr *a, int nComp, cons
     if (a->nCFaces == 0) return B200LDU_OK;
     if (!pnf_d) return B200LDU_EINVAL;
     double *send = nullptr;
-    TRY(scratch(a, 3, (size_t)a->nCFaces * nComp, &send));
+    TRY(a->mem.slot(ADDR_FVM_CMPT_PSI, send, (size_t)a->nCFaces * nComp));
     fieldk::gather_kernel<<<grid(a->nCFaces * nComp, 256), 256, 0, a->ctx->stream>>>(a->nCFaces, nComp, a->d_cFaceCells,
                                                                                       field_d, send);
     a->ctx->launches++;
@@ -241,7 +227,7 @@ extern "C" int b200ldu_fvm_residual(b200ldu_matrix *m, const double *psi_d, cons
         return B200LDU_EINVAL;
     }
     double *tmp = nullptr;
-    TRY(scratch(a, 0, (size_t)a->nCells, &tmp));
+    TRY(a->mem.slot(ADDR_FVM_DIAG, tmp, (size_t)a->nCells));
     residual_source_kernel<<<grid(a->nCells, 256), 256, 0, a->ctx->stream>>>(a->nCells, L, internalCoeffs_d, m->int_ext,
                                                                              psi_d, source_d, tmp);
     a->ctx->launches++;
@@ -312,8 +298,8 @@ extern "C" int b200ldu_fvm_solve(b200ldu_matrix *m, int nComp, const char *solve
     const double *diag0 = m->diag_ext;
     const double *bou = m->bou_ext, *intc = m->int_ext;
     double *dK = nullptr, *total = nullptr, *sK = nullptr, *pK = nullptr;
-    TRY(scratch(a, 0, (size_t)n, &dK));
-    TRY(scratch(a, 1, (size_t)n * nComp, &total));
+    TRY(a->mem.slot(ADDR_FVM_DIAG, dK, (size_t)n));
+    TRY(a->mem.slot(ADDR_FVM_SOURCE, total, (size_t)n * nComp));
     int rc = B200LDU_OK;
     if (nComp == 1) {
         boundary_diag_kernel<<<grid(n, 256), 256, 0, st>>>(n, L, internalCoeffs_d, 1, 0, intc, diag0, dK);
@@ -323,8 +309,8 @@ extern "C" int b200ldu_fvm_solve(b200ldu_matrix *m, int nComp, const char *solve
         rc = matrix_set_diag(m, dK); // the off-diagonal streams are unchanged
         if (rc == B200LDU_OK) rc = b200ldu_solve(m, solver, precondOrSmoother, controls, gamg, psi_d, total, &perf[0], nullptr, 0);
     } else {
-        TRY(scratch(a, 2, (size_t)n, &sK));
-        TRY(scratch(a, 3, (size_t)n, &pK));
+        TRY(a->mem.slot(ADDR_FVM_CMPT_SOURCE, sK, (size_t)n));
+        TRY(a->mem.slot(ADDR_FVM_CMPT_PSI, pK, (size_t)n));
         boundary_source_kernel<3><<<grid(n, 256), 256, 0, st>>>(n, L, boundaryCoeffs_d, bou, pnf_d, source_d, total);
         a->ctx->launches++;
         KERNEL_CHECK();

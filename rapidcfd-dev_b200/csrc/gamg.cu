@@ -68,11 +68,16 @@ struct GamgLevel {
     double *corr = nullptr, *src = nullptr, *tmp = nullptr, *acf = nullptr, *pre = nullptr;
 };
 
+// slots of b200ldu_gamg::mem
+enum GamgSlot { GAMG_INV, GAMG_GATHER };
+
 struct b200ldu_gamg {
+    explicit b200ldu_gamg(b200ldu_addr *a) : finest(a), mem(a->ctx) {}
     b200ldu_addr *finest = nullptr;
+    DeviceMem mem; // the levels' device arrays (fixed) and the coarsest-level solve's (slots); the levels' addressings
+                   // and matrices own theirs
     int nLevels = 0;
     std::vector<GamgLevel> lev;
-    std::vector<void *> mem; // every device array the levels' set-up allocated (dev_alloc, upload)
     double *d_inv = nullptr; // this rank's rows of the inverse of the (global) coarsest matrix
     int invN = 0;            // global size of the coarsest system
     // multi-rank coarsest solve
@@ -395,21 +400,21 @@ static int level_upload(b200ldu_gamg *g, const b200ldu_addr *fineAddr, GamgHostL
     TRY(b200ldu_addr_create(a->ctx, nCoarse, H.nCoarseFaces, H.cOwner.data(), H.cNeigh.data(), nPatches,
                             nPatches ? L.cPatchStart.data() : nullptr, nPatches ? L.cFaceCells.data() : nullptr,
                             nPatches ? a->neighbRank.data() : nullptr, H.cc.empty() ? nullptr : H.cc.data(), &L.addr));
-    std::vector<void *> &mem = g->mem;
+    DeviceMem &mem = g->mem;
     if (nPatches) {
         std::vector<int> ps, pi;
         csr_from_map(H.pfRestrict, H.nCoarsePF, ps, pi);
-        TRY(upload(mem, L.d_pfChildStart, ps));
-        TRY(upload(mem, L.d_pfChild, pi));
-        TRY(dev_alloc(mem, L.d_bou, H.nCoarsePF));
-        TRY(dev_alloc(mem, L.d_int, H.nCoarsePF));
+        TRY(mem.upload(L.d_pfChildStart, ps));
+        TRY(mem.upload(L.d_pfChild, pi));
+        TRY(mem.alloc(L.d_bou, H.nCoarsePF));
+        TRY(mem.alloc(L.d_int, H.nCoarsePF));
     }
     TRY(b200ldu_matrix_create(L.addr, &L.mat));
     // caller order: coarse cell -> fine cells ascending
     std::vector<int> cs, ci;
     csr_from_map(L.restrictAddr, nCoarse, cs, ci);
-    TRY(upload(mem, L.d_cellChildStart, cs));
-    TRY(upload(mem, L.d_cellChild, ci));
+    TRY(mem.upload(L.d_cellChildStart, cs));
+    TRY(mem.upload(L.d_cellChild, ci));
     // banded: coarse row -> fine rows, fine row -> coarse row
     const std::vector<int> &finePerm = fineAddr->perm_h, &fiperm = fineAddr->iperm_h;
     const std::vector<int> &cperm = L.addr->perm_h, &ciperm = L.addr->iperm_h;
@@ -424,9 +429,9 @@ static int level_upload(b200ldu_gamg *g, const b200ldu_addr *fineAddr, GamgHostL
     std::vector<int> pm(nPadF, -1);
     for (int q = 0; q < nPadF; q++)
         if (fiperm[q] >= 0) pm[q] = cperm[L.restrictAddr[fiperm[q]]];
-    TRY(upload(mem, L.d_childStart, bs));
-    TRY(upload(mem, L.d_child, bi));
-    TRY(upload(mem, L.d_pmap, pm));
+    TRY(mem.upload(L.d_childStart, bs));
+    TRY(mem.upload(L.d_child, bi));
+    TRY(mem.upload(L.d_pmap, pm));
     // face maps (caller order): coarse face -> (fine face << 1 | flip), coarse cell -> collapsed fine faces
     std::vector<int> fmap(H.nFineFaces), dmap(H.nFineFaces);
     for (int f = 0; f < H.nFineFaces; f++) {
@@ -437,15 +442,15 @@ static int level_upload(b200ldu_gamg *g, const b200ldu_addr *fineAddr, GamgHostL
     csr_from_map(fmap, H.nCoarseFaces, fs, fi);
     csr_from_map(dmap, nCoarse, ds, di);
     for (int k = 0; k < fs[H.nCoarseFaces]; k++) fi[k] = (fi[k] << 1) | (H.faceFlip[fi[k]] ? 1 : 0);
-    TRY(upload(mem, L.d_faceChildStart, fs));
-    TRY(upload(mem, L.d_faceChild, fi));
-    TRY(upload(mem, L.d_diagFaceStart, ds));
-    TRY(upload(mem, L.d_diagFace, di));
-    TRY(dev_alloc(mem, L.d_diag, nCoarse));
-    TRY(dev_alloc(mem, L.d_upper, H.nCoarseFaces));
-    TRY(dev_alloc(mem, L.d_lower, H.nCoarseFaces));
+    TRY(mem.upload(L.d_faceChildStart, fs));
+    TRY(mem.upload(L.d_faceChild, fi));
+    TRY(mem.upload(L.d_diagFaceStart, ds));
+    TRY(mem.upload(L.d_diagFace, di));
+    TRY(mem.alloc(L.d_diag, nCoarse));
+    TRY(mem.alloc(L.d_upper, H.nCoarseFaces));
+    TRY(mem.alloc(L.d_lower, H.nCoarseFaces));
     for (double **v : {&L.corr, &L.src, &L.tmp, &L.acf, &L.pre}) {
-        TRY(dev_alloc(mem, *v, L.addr->vecLen));
+        TRY(mem.alloc(*v, L.addr->vecLen));
         CUDA_TRY(cudaMemsetAsync(*v, 0, sizeof(double) * (size_t)L.addr->vecLen, a->ctx->stream));
     }
     return B200LDU_OK;
@@ -461,11 +466,8 @@ extern "C" int b200ldu_gamg_destroy(b200ldu_gamg *g)
             if (L.mat) b200ldu_matrix_destroy(L.mat);
             if (L.addr) b200ldu_addr_destroy(L.addr);
         }
-        for (void *p : g->mem) cudaFree(p);
-        if (g->d_inv) cudaFree(g->d_inv);
-        if (g->d_gatherAll) cudaFree(g->d_gatherAll);
     }
-    delete g;
+    delete g; // its DeviceMem frees every device array (a host-only hierarchy has none)
     return B200LDU_OK;
 }
 
@@ -495,8 +497,7 @@ extern "C" int b200ldu_gamg_create(b200ldu_addr *a, const double *faceWeights_h,
     std::vector<GamgHostLevel> H;
     int rc = agglomerate(a, faceWeights_h, nCellsInCoarsestLevel, mergeLevels, forward, H);
     if (forwardInOut) *forwardInOut = forward ? 1 : 0;
-    b200ldu_gamg *g = new b200ldu_gamg();
-    g->finest = a;
+    b200ldu_gamg *g = new b200ldu_gamg(a);
     if (rc == B200LDU_OK && !H.empty() && !a->hostOnly) rc = coarsest_setup(g, a, H.back());
     for (size_t k = 0; k < H.size() && rc == B200LDU_OK; k++)
         rc = level_upload(g, k ? g->lev[k - 1].addr : a, std::move(H[k]));
@@ -858,16 +859,11 @@ static int gamg_coarsest_inverse(Solve &S, b200ldu_gamg *g)
             }
         }
     }
-    size_t need = (size_t)std::max(n, 1) * N;
-    if ((size_t)g->invN * g->invN < need || !g->d_inv) {
-        if (g->d_inv) cudaFree(g->d_inv);
-        g->d_inv = nullptr;
-        CUDA_TRY(cudaMalloc((void **)&g->d_inv, sizeof(double) * need));
-    }
+    TRY(g->mem.slot(GAMG_INV, g->d_inv, (size_t)std::max(n, 1) * N));
     g->invN = N;
     CUDA_TRY(cudaMemcpyAsync(g->d_inv, &I[(size_t)off * N], sizeof(double) * (size_t)n * N, cudaMemcpyHostToDevice, st));
-    if (R > 1 && !ctx->p2p && !g->d_gatherAll)
-        CUDA_TRY(cudaMalloc((void **)&g->d_gatherAll, sizeof(double) * (size_t)(R + 1) * P2P_GMAX + sizeof(int) * 64));
+    if (R > 1 && !ctx->p2p) // the gathered right-hand sides, then 64 ints of rank offsets and counts
+        TRY(g->mem.slot(GAMG_GATHER, g->d_gatherAll, (size_t)(R + 1) * P2P_GMAX + 32));
     CUDA_TRY(cudaStreamSynchronize(st)); // I goes out of scope
     return B200LDU_OK;
 }

@@ -61,6 +61,94 @@ struct b200ldu_ctx {
     char *region = nullptr;          // this rank's shared region
     char *peerRegion[8] = {nullptr}; // every rank's region mapped here (own included)
     unsigned long long *d_seq = nullptr; // local device counters: [0] reduction seq, [1] halo seq, [2..] scratch
+    // device memory of the handles created on this context (DeviceMem): bytes held, allocations made
+    long long memLive = 0, memAllocs = 0;
+};
+
+// Device memory of one handle (addressing, matrix, GAMG hierarchy): every device array the handle holds is allocated
+// here and freed with the handle.  Fixed arrays live as long as the handle; numbered slots grow on demand and never
+// shrink.  The contents of a slot are unspecified after it was reallocated, except that zeroNew zeroes a new
+// allocation on the context's stream.
+class DeviceMem {
+  public:
+    explicit DeviceMem(b200ldu_ctx *ctx) : ctx_(ctx) {}
+    ~DeviceMem()
+    {
+        for (Block &b : fixed_) free_(b);
+        for (Block &b : slots_) free_(b);
+    }
+    DeviceMem(const DeviceMem &) = delete;
+    DeviceMem &operator=(const DeviceMem &) = delete;
+
+    // fixed array of n (at least one) T
+    template <class T>
+    int alloc(T *&d, size_t n)
+    {
+        fixed_.emplace_back();
+        return grow(fixed_.back(), d, n, false);
+    }
+    // slot k viewed through d, holding at least n (at least one) T: reallocated only when n is larger than it holds
+    template <class T>
+    int slot(int k, T *&d, size_t n, bool zeroNew = false)
+    {
+        if ((int)slots_.size() <= k) slots_.resize(k + 1);
+        return grow(slots_[k], d, n, zeroNew);
+    }
+    // h uploaded into a new fixed array, or into slot k
+    template <class Ptr, class T>
+    int upload(Ptr &d, const std::vector<T> &h)
+    {
+        T *p = nullptr;
+        TRY(alloc(p, h.size()));
+        d = p;
+        return copy_in(p, h);
+    }
+    template <class T>
+    int upload(int k, T *&d, const std::vector<T> &h)
+    {
+        TRY(slot(k, d, h.size()));
+        return copy_in(d, h);
+    }
+    void release(int k)
+    {
+        if (k < (int)slots_.size()) free_(slots_[k]);
+    }
+
+  private:
+    struct Block {
+        void *p = nullptr;
+        size_t bytes = 0;
+    };
+    template <class T>
+    int grow(Block &b, T *&d, size_t n, bool zeroNew)
+    {
+        const size_t bytes = sizeof(T) * (n ? n : 1);
+        if (b.bytes < bytes) {
+            free_(b);
+            d = nullptr;
+            CUDA_TRY(cudaMalloc(&b.p, bytes));
+            b.bytes = bytes;
+            ctx_->memLive += (long long)bytes;
+            ctx_->memAllocs++;
+            if (zeroNew) CUDA_TRY(cudaMemsetAsync(b.p, 0, bytes, ctx_->stream));
+        }
+        d = (T *)b.p;
+        return B200LDU_OK;
+    }
+    void free_(Block &b)
+    {
+        if (b.bytes) cudaFree(b.p); // bytes is set once cudaMalloc succeeded
+        ctx_->memLive -= (long long)b.bytes;
+        b = Block();
+    }
+    template <class T>
+    static int copy_in(T *d, const std::vector<T> &h)
+    {
+        if (h.size()) CUDA_TRY(cudaMemcpy(d, h.data(), sizeof(T) * h.size(), cudaMemcpyHostToDevice));
+        return B200LDU_OK;
+    }
+    b200ldu_ctx *ctx_;
+    std::vector<Block> fixed_, slots_;
 };
 
 // layout of the IPC-shared region of every rank
@@ -166,8 +254,20 @@ struct LayoutHost {
     std::vector<int> fsCode, fsListStart, fsListIfc;
 };
 
+// slots of b200ldu_addr::mem
+enum AddrSlot {
+    ADDR_X, ADDR_Y, ADDR_B,                              // banded vectors of the caller-order entry points (ldu.cu)
+    ADDR_BFACE_CELLS, ADDR_BCELL_START, ADDR_BCELL_FACES, // boundary face lists (b200ldu_fv_boundary_set)
+    // fvMatrix glue (fvmatrix.cu): cell fields of fvm_solve / fvm_residual, and the patch-face send buffer of
+    // fv_patch_neighbour_field, which shares its slot with the component psi of fvm_solve
+    ADDR_FVM_DIAG, ADDR_FVM_SOURCE, ADDR_FVM_CMPT_SOURCE, ADDR_FVM_CMPT_PSI,
+    ADDR_MULES, // MULES limiter: six cell fields and the received limiters (mules.cu)
+};
+
 struct b200ldu_addr {
+    explicit b200ldu_addr(b200ldu_ctx *c) : ctx(c), mem(c) {}
     b200ldu_ctx *ctx = nullptr;
+    DeviceMem mem; // every device array below (fixed: the layout, cyclic sources, halo send and coupled-face lists)
     int nCells = 0, nFaces = 0;
     std::vector<int> l, u; // host copies (GAMG agglomeration, FV CSR build)
     int nPatches = 0;
@@ -178,44 +278,47 @@ struct b200ldu_addr {
     long long nHaloTotal = 0;
     std::vector<int> perm_h, iperm_h;
     std::vector<double> centres_h; // optional cell centres (kept for GAMG coarse-level banding)
-    // device arrays owned: layoutMem holds every array layout_build uploaded (L's arrays, d_code, d_fsCode and the
-    // caller-order CSR views d_l .. d_losortStart); the other pointers below own their arrays
-    std::vector<void *> layoutMem;
     int *d_code = nullptr; // [nEntries] value source: 2f+side | -1 pad | -2-pf interface
     // face stream: used by symmetric matrices when the layout has one (hasFs)
     bool hasFs = false;
     long long fsOwn = 0, fsList = 0; // stored owner slots (padding included), list items
     int *d_fsCode = nullptr; // [fsOwn + fsList] value source, as d_code
     bool p2pHalo = false;      // peer-store halo usable for this addressing
-    void *d_packPatches = nullptr, *d_packChunks = nullptr; // PackPatch[], PackChunk[] (comm.cu)
-    int nPackChunks = 0;
     double nCellsGlobal = 0;
     // caller-order CSR views for the FV face-sum kernels and faceH
     int *d_cyclicSrc = nullptr; // per coupled-patch face: banded row supplying it (cyclic partner) | -1
     int *d_l = nullptr, *d_u = nullptr, *d_ownerStart = nullptr, *d_losort = nullptr,
         *d_losortStart = nullptr;
+    // boundary faces (all patches, patch order) and their per-cell lists; the lists are valid for nBFaces > 0 only
     int nBFaces = 0;
-    int *d_bFaceCells = nullptr;    // boundary faces (all patches, patch order)
-    int *d_bCellStart = nullptr, *d_bCellFaces = nullptr, *d_bCells = nullptr; // per boundary cell lists
-    int nBCells = 0;
-    // fvMatrix glue (fvmatrix.cu): per-cell lists over the coupled patch faces, built at first use, and
-    // grow-only scratch vectors
+    int *d_bFaceCells = nullptr;
+    int *d_bCellStart = nullptr, *d_bCellFaces = nullptr;
+    // fvMatrix glue (fvmatrix.cu): per-cell lists over the coupled patch faces, built at first use
     int nCFaces = 0;
     int *d_cCellStart = nullptr, *d_cCellFaces = nullptr, *d_cFaceCells = nullptr;
-    double *d_mulesScratch = nullptr; // MULES limiter: six cell fields (mules.cu)
-    size_t mulesScratchLen = 0;
-    double *d_fvmScratch[4] = {nullptr, nullptr, nullptr, nullptr};
-    size_t fvmScratchLen[4] = {0, 0, 0, 0};
     // host-only structural self-check (b200ldu_layout_debug_*): no GPU, no compute
     bool hostOnly = false;
     LayoutHost host;
-    // workspace pool for caller-order entry points (banded vectors)
-    std::vector<double *> pool;
     long long vecLen = 0; // nPad + nRecv (padded to even)
 };
 
+// slots of b200ldu_matrix::mem
+enum MatSlot {
+    MAT_WORK,                        // solver work vectors MAT_WORK + [0, MAT_NWORK) (Solve::vec; solvers.cu, gamg.cu)
+    MAT_NWORK = 8,
+    MAT_PSI = MAT_WORK + MAT_NWORK,  // banded psi / source of b200ldu_solve
+    MAT_SRC,
+    MAT_HOST_PSI, MAT_HOST_SRC,      // caller-order psi / source of b200ldu_solve_host
+    MAT_HIST,                        // device residual history
+    MAT_OWN_DIAG, MAT_OWN_UPPER, MAT_OWN_LOWER, MAT_OWN_BOU, MAT_OWN_INT, // caller-order copies (matrix_set)
+    MAT_VAL, MAT_VALT, MAT_FVAL,     // coefficient streams (matrix_set)
+};
+
 struct b200ldu_matrix {
+    explicit b200ldu_matrix(b200ldu_addr *addr) : a(addr), mem(addr->ctx) {}
     b200ldu_addr *a = nullptr;
+    DeviceMem mem; // every device array below; the workspace slots are allocated once and reused across solves
+                   // (PCGCache.H:9-58)
     bool symmetric = true;
     bool haveT = false;
     double *d_val = nullptr;  // banded coefficients for Amul   [nEntries]
@@ -223,55 +326,26 @@ struct b200ldu_matrix {
     double *d_fval = nullptr; // face-stream coefficients [fsOwn + fsList]: a symmetric matrix has these instead of d_val
     double *d_diag = nullptr; // banded diagonal [nPad] (padding rows = 1)
     double *d_rD = nullptr;   // 1/diag, filled by matrix_set
-    // caller-order coefficients OWNED by the matrix (copied by matrix_set): diag, upper, lower, interfaceBouCoeffs,
-    // interfaceIntCoeffs -- read by faceH, the fvMatrix glue and the GAMG coarse-level assembly
-    double *own[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
-    size_t ownLen[5] = {0, 0, 0, 0, 0};
-    // current views of them (diag_ext is re-pointed at the boundary-folded diagonal for the duration of fvm_solve;
-    // lower_ext aliases upper_ext when symmetric, int_ext aliases bou_ext when the caller passed one array for both)
+    // views of the caller-order coefficients the matrix owns (copied by matrix_set) -- read by faceH, the fvMatrix
+    // glue and the GAMG coarse-level assembly.  diag_ext is re-pointed at the boundary-folded diagonal for the
+    // duration of fvm_solve; lower_ext aliases upper_ext when symmetric, int_ext aliases bou_ext when the caller
+    // passed one array for both.
     const double *upper_ext = nullptr, *lower_ext = nullptr, *diag_ext = nullptr, *bou_ext = nullptr,
                  *int_ext = nullptr;
-    // solver workspace (allocated once, reused across solves -- PCGCache.H:9-58)
-    std::vector<double *> work;
     double *d_partials = nullptr; // reduction partials
     void *d_scal = nullptr;       // SolverScalars
-    double *d_hist = nullptr;     // device residual history
     double *d_sendBuf = nullptr;  // packed psi at coupled-patch face cells
-    int histCap = 0;
 };
 
 // ---------------------------------------------------------------------------
 // cross-file helpers
 // ---------------------------------------------------------------------------
 int layout_build(b200ldu_addr *a, const double *centres);
-int addr_alloc_vec(b200ldu_addr *a, double **out); // banded vector of vecLen doubles, zeroed
-double *addr_pool_vec(b200ldu_addr *a, int slot);  // reusable scratch (grows on demand)
 
-template <class T>
-int dev_upload(T **d, const std::vector<T> &h)
+// banded vector of a's vecLen doubles in slot k of mem, zeroed when first allocated (its padding rows and receive tail
+// rely on it); nullptr when the allocation fails
+inline double *banded_vec(const b200ldu_addr *a, DeviceMem &mem, int k)
 {
-    size_t bytes = sizeof(T) * (h.size() ? h.size() : 1);
-    CUDA_TRY(cudaMalloc((void **)d, bytes));
-    if (h.size()) CUDA_TRY(cudaMemcpy(*d, h.data(), sizeof(T) * h.size(), cudaMemcpyHostToDevice));
-    return B200LDU_OK;
-}
-
-// device array of n (at least one) T, recorded in mem, whose owner frees every pointer in it
-template <class T>
-int dev_alloc(std::vector<void *> &mem, T *&d, size_t n)
-{
-    CUDA_TRY(cudaMalloc((void **)&d, sizeof(T) * (n ? n : 1)));
-    mem.push_back(d);
-    return B200LDU_OK;
-}
-
-// uploads h into a new device array recorded in mem
-template <class Ptr, class T>
-int upload(std::vector<void *> &mem, Ptr &d, const std::vector<T> &h)
-{
-    T *p = nullptr;
-    TRY(dev_alloc(mem, p, h.size()));
-    d = p;
-    if (h.size()) CUDA_TRY(cudaMemcpy(p, h.data(), sizeof(T) * h.size(), cudaMemcpyHostToDevice));
-    return B200LDU_OK;
+    double *d = nullptr;
+    return mem.slot(k, d, (size_t)a->vecLen, true) == B200LDU_OK ? d : nullptr;
 }

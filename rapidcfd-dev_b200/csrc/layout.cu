@@ -547,33 +547,32 @@ void fill_face_stream(const Graph &g, const std::vector<int> &perm, Plan &P)
     }
 }
 
-// ---- 8. device path: upload the record (into a->layoutMem, which b200ldu_addr_destroy frees), set every layout
-// field of the addressing ----
+// ---- 8. device path: upload the record into fixed arrays of the addressing, set every layout field of it ----
 int layout_upload(b200ldu_addr *a, const Graph &g, const LayoutHost &H)
 {
     LayoutDev &L = a->L;
-    std::vector<void *> &mem = a->layoutMem;
-    TRY(upload(mem, L.sliceStart, H.sliceStart));
-    TRY(upload(mem, L.sliceW, H.sliceW));
-    TRY(upload(mem, L.sliceWL, H.sliceWL));
-    TRY(upload(mem, L.col, H.col));
-    TRY(upload(mem, a->d_code, H.code));
-    TRY(upload(mem, L.haloStart, H.haloStart));
-    TRY(upload(mem, L.haloIdx, H.haloIdx));
-    TRY(upload(mem, L.perm, a->perm_h));
-    TRY(upload(mem, L.iperm, a->iperm_h));
-    TRY(upload(mem, L.sendRows, H.sendRows));
-    TRY(upload(mem, a->d_l, a->l));
-    TRY(upload(mem, a->d_u, a->u));
-    TRY(upload(mem, a->d_ownerStart, g.ownerStart));
-    TRY(upload(mem, a->d_losort, g.losort));
-    TRY(upload(mem, a->d_losortStart, g.losortStart));
+    DeviceMem &mem = a->mem;
+    TRY(mem.upload(L.sliceStart, H.sliceStart));
+    TRY(mem.upload(L.sliceW, H.sliceW));
+    TRY(mem.upload(L.sliceWL, H.sliceWL));
+    TRY(mem.upload(L.col, H.col));
+    TRY(mem.upload(a->d_code, H.code));
+    TRY(mem.upload(L.haloStart, H.haloStart));
+    TRY(mem.upload(L.haloIdx, H.haloIdx));
+    TRY(mem.upload(L.perm, a->perm_h));
+    TRY(mem.upload(L.iperm, a->iperm_h));
+    TRY(mem.upload(L.sendRows, H.sendRows));
+    TRY(mem.upload(a->d_l, a->l));
+    TRY(mem.upload(a->d_u, a->u));
+    TRY(mem.upload(a->d_ownerStart, g.ownerStart));
+    TRY(mem.upload(a->d_losort, g.losort));
+    TRY(mem.upload(a->d_losortStart, g.losortStart));
     if (H.hasFs) {
-        TRY(upload(mem, L.fsSlice, H.fsSlice));
-        TRY(upload(mem, L.fsCT, H.fsCT));
-        TRY(upload(mem, a->d_fsCode, H.fsCode));
-        TRY(upload(mem, L.fsListStart, H.fsListStart));
-        TRY(upload(mem, L.fsListIfc, H.fsListIfc));
+        TRY(mem.upload(L.fsSlice, H.fsSlice));
+        TRY(mem.upload(L.fsCT, H.fsCT));
+        TRY(mem.upload(a->d_fsCode, H.fsCode));
+        TRY(mem.upload(L.fsListStart, H.fsListStart));
+        TRY(mem.upload(L.fsListIfc, H.fsListIfc));
     }
     L.nCells = g.nCells;
     L.nPad = H.nPad;
@@ -652,7 +651,7 @@ extern "C" int b200ldu_layout_debug_create(int nCells, int nFaces, const int *lo
                                            const double *cellCentres_h, b200ldu_addr **out)
 {
     if (!out || nCells <= 0) return B200LDU_EINVAL;
-    b200ldu_addr *a = new b200ldu_addr();
+    b200ldu_addr *a = new b200ldu_addr(nullptr);
     a->hostOnly = true;
     a->nCells = nCells;
     a->nFaces = nFaces;

@@ -105,6 +105,14 @@ extern "C" int b200ldu_ctx_sync(b200ldu_ctx *c)
 
 extern "C" long long b200ldu_launch_count(const b200ldu_ctx *c) { return c ? c->launches : 0; }
 
+extern "C" int b200ldu_ctx_device_mem(const b200ldu_ctx *c, long long *liveBytes, long long *nAllocs)
+{
+    if (!c) return B200LDU_EINVAL;
+    if (liveBytes) *liveBytes = c->memLive;
+    if (nAllocs) *nAllocs = c->memAllocs;
+    return B200LDU_OK;
+}
+
 int ctx_pinned(b200ldu_ctx *c, size_t bytes, void **out)
 {
     if (bytes > c->pinnedBytes) {
@@ -121,6 +129,31 @@ int ctx_pinned(b200ldu_ctx *c, size_t bytes, void **out)
 // ---------------------------------------------------------------------------
 // addressing
 // ---------------------------------------------------------------------------
+// cyclic patches: neighbRank[p] = -(q+1) pairs patch p with patch q of this addressing, face i
+// with face i (cyclicLduInterface: neighbPatchID).  Their "received" values are psi at the
+// partner's face cells, copied on the device (comm_halo_exchange).
+static int cyclic_setup(b200ldu_addr *a)
+{
+    const int nPatches = a->nPatches;
+    bool any = false;
+    for (int p = 0; p < nPatches; p++) any = any || a->neighbRank[p] < 0;
+    if (!any) return B200LDU_OK;
+    std::vector<int> src((size_t)a->patchStart[nPatches], -1);
+    for (int p = 0; p < nPatches; p++) {
+        if (a->neighbRank[p] >= 0) continue;
+        const int q = -a->neighbRank[p] - 1;
+        const int n = a->patchStart[p + 1] - a->patchStart[p];
+        if (q < 0 || q >= nPatches || q == p || a->neighbRank[q] != -(p + 1) ||
+            a->patchStart[q + 1] - a->patchStart[q] != n) {
+            b200_set_error("addr_create: cyclic patch %d has no matching partner patch", p);
+            return B200LDU_EINVAL;
+        }
+        for (int i = 0; i < n; i++)
+            src[(size_t)a->patchStart[p] + i] = a->perm_h[a->faceCells[(size_t)a->patchStart[q] + i]];
+    }
+    return a->mem.upload(a->d_cyclicSrc, src);
+}
+
 extern "C" int b200ldu_addr_create(b200ldu_ctx *ctx, int nCells, int nFaces, const int *lower_h,
                                    const int *upper_h, int nPatches, const int *patchStart_h,
                                    const int *faceCells_h, const int *neighbRank_h,
@@ -131,9 +164,13 @@ extern "C" int b200ldu_addr_create(b200ldu_ctx *ctx, int nCells, int nFaces, con
         b200_set_error("addr_create: bad arguments");
         return B200LDU_EINVAL;
     }
+    for (int i = 0; nPatches && i < patchStart_h[nPatches]; i++)
+        if (faceCells_h[i] < 0 || faceCells_h[i] >= nCells) {
+            b200_set_error("addr_create: patch faceCells out of range");
+            return B200LDU_EINVAL;
+        }
     CUDA_TRY(cudaSetDevice(ctx->device));
-    b200ldu_addr *a = new b200ldu_addr();
-    a->ctx = ctx;
+    b200ldu_addr *a = new b200ldu_addr(ctx);
     a->nCells = nCells;
     a->nFaces = nFaces;
     a->l.assign(lower_h, lower_h + nFaces);
@@ -143,52 +180,14 @@ extern "C" int b200ldu_addr_create(b200ldu_ctx *ctx, int nCells, int nFaces, con
         a->patchStart.assign(patchStart_h, patchStart_h + nPatches + 1);
         a->faceCells.assign(faceCells_h, faceCells_h + a->patchStart[nPatches]);
         a->neighbRank.assign(neighbRank_h, neighbRank_h + nPatches);
-        for (int i = 0; i < a->patchStart[nPatches]; i++)
-            if (a->faceCells[i] < 0 || a->faceCells[i] >= nCells) {
-                b200_set_error("addr_create: patch faceCells out of range");
-                delete a;
-                return B200LDU_EINVAL;
-            }
     }
     if (cellCentres_h) a->centres_h.assign(cellCentres_h, cellCentres_h + 3 * (size_t)nCells);
     int rc = layout_build(a, cellCentres_h);
+    if (rc == B200LDU_OK) rc = comm_addr_setup(a);
+    if (rc == B200LDU_OK) rc = cyclic_setup(a);
     if (rc != B200LDU_OK) {
         b200ldu_addr_destroy(a);
         return rc;
-    }
-    rc = comm_addr_setup(a);
-    if (rc != B200LDU_OK) {
-        b200ldu_addr_destroy(a);
-        return rc;
-    }
-    // cyclic patches: neighbRank[p] = -(q+1) pairs patch p with patch q of this addressing, face i
-    // with face i (cyclicLduInterface: neighbPatchID).  Their "received" values are psi at the
-    // partner's face cells, copied on the device (comm_halo_exchange).
-    {
-        bool any = false;
-        for (int p = 0; p < nPatches; p++) any = any || a->neighbRank[p] < 0;
-        if (any) {
-            std::vector<int> src((size_t)a->patchStart[nPatches], -1);
-            for (int p = 0; p < nPatches; p++) {
-                if (a->neighbRank[p] >= 0) continue;
-                const int q = -a->neighbRank[p] - 1;
-                const int n = a->patchStart[p + 1] - a->patchStart[p];
-                if (q < 0 || q >= nPatches || q == p || a->neighbRank[q] != -(p + 1) ||
-                    a->patchStart[q + 1] - a->patchStart[q] != n) {
-                    b200_set_error("addr_create: cyclic patch %d has no matching partner patch", p);
-                    b200ldu_addr_destroy(a);
-                    return B200LDU_EINVAL;
-                }
-                for (int i = 0; i < n; i++)
-                    src[(size_t)a->patchStart[p] + i] = a->perm_h[a->faceCells[(size_t)a->patchStart[q] + i]];
-            }
-            if (cudaMalloc((void **)&a->d_cyclicSrc, sizeof(int) * src.size()) != cudaSuccess ||
-                cudaMemcpy(a->d_cyclicSrc, src.data(), sizeof(int) * src.size(), cudaMemcpyHostToDevice) != cudaSuccess) {
-                b200_set_error("addr_create: out of device memory");
-                b200ldu_addr_destroy(a);
-                return B200LDU_ECUDA;
-            }
-        }
     }
     *out = a;
     return B200LDU_OK;
@@ -199,16 +198,7 @@ extern "C" int b200ldu_addr_destroy(b200ldu_addr *a)
     if (!a) return B200LDU_OK;
     cudaSetDevice(a->ctx->device);
     cudaStreamSynchronize(a->ctx->stream);
-    void *ptrs[] = {a->d_bFaceCells, a->d_cyclicSrc, a->d_bCellStart, a->d_bCellFaces, a->d_bCells,
-                    a->d_packPatches, a->d_packChunks, a->d_cCellStart, a->d_cCellFaces, a->d_cFaceCells,
-                    a->d_mulesScratch, a->d_fvmScratch[0], a->d_fvmScratch[1], a->d_fvmScratch[2],
-                    a->d_fvmScratch[3]};
-    for (void *p : ptrs)
-        if (p) cudaFree(p);
-    for (void *p : a->layoutMem) cudaFree(p);
-    for (double *p : a->pool)
-        if (p) cudaFree(p);
-    delete a;
+    delete a; // its DeviceMem frees every device array
     return B200LDU_OK;
 }
 
@@ -243,22 +233,6 @@ extern "C" int b200ldu_addr_perm(const b200ldu_addr *a, int *perm_h)
 }
 
 extern "C" long long b200ldu_vec_len(const b200ldu_addr *a) { return a ? a->vecLen : 0; }
-
-int addr_alloc_vec(b200ldu_addr *a, double **out)
-{
-    CUDA_TRY(cudaMalloc((void **)out, sizeof(double) * (size_t)a->vecLen));
-    CUDA_TRY(cudaMemsetAsync(*out, 0, sizeof(double) * (size_t)a->vecLen, a->ctx->stream));
-    return B200LDU_OK;
-}
-
-double *addr_pool_vec(b200ldu_addr *a, int slot)
-{
-    while ((int)a->pool.size() <= slot) a->pool.push_back(nullptr);
-    if (!a->pool[slot]) {
-        if (addr_alloc_vec(a, &a->pool[slot]) != B200LDU_OK) return nullptr;
-    }
-    return a->pool[slot];
-}
 
 // ---- caller order <-> banded order ----
 __global__ void to_banded_kernel(int nPad, const int *__restrict__ iperm, const double *__restrict__ x,
@@ -314,16 +288,24 @@ extern "C" int b200ldu_matrix_create(b200ldu_addr *a, b200ldu_matrix **out)
 {
     if (!a || !out) return B200LDU_EINVAL;
     CUDA_TRY(cudaSetDevice(a->ctx->device));
-    b200ldu_matrix *m = new b200ldu_matrix();
-    m->a = a;
+    b200ldu_matrix *m = new b200ldu_matrix(a);
     // coefficient streams are allocated by matrix_set (which layout is used depends on symmetry)
-    CUDA_TRY(cudaMalloc((void **)&m->d_diag, sizeof(double) * (size_t)a->vecLen));
-    CUDA_TRY(cudaMalloc((void **)&m->d_rD, sizeof(double) * (size_t)a->vecLen));
-    int np = a->L.nBands > a->ctx->smCount * 8 ? a->L.nBands : a->ctx->smCount * 8;
-    CUDA_TRY(cudaMalloc((void **)&m->d_partials, sizeof(double) * 4 * (size_t)np));
-    CUDA_TRY(cudaMalloc((void **)&m->d_scal, sizeof(SolverScalars)));
-    CUDA_TRY(cudaMemset(m->d_scal, 0, sizeof(SolverScalars)));
-    CUDA_TRY(cudaMalloc((void **)&m->d_sendBuf, sizeof(double) * (size_t)(a->L.nRecv > 0 ? a->L.nRecv : 1)));
+    auto alloc = [&]() -> int {
+        const int np = a->L.nBands > a->ctx->smCount * 8 ? a->L.nBands : a->ctx->smCount * 8;
+        SolverScalars *scal = nullptr;
+        TRY(m->mem.alloc(m->d_diag, (size_t)a->vecLen));
+        TRY(m->mem.alloc(m->d_rD, (size_t)a->vecLen));
+        TRY(m->mem.alloc(m->d_partials, 4 * (size_t)np));
+        TRY(m->mem.alloc(scal, 1));
+        CUDA_TRY(cudaMemset(scal, 0, sizeof(SolverScalars)));
+        m->d_scal = scal;
+        return m->mem.alloc(m->d_sendBuf, (size_t)a->L.nRecv);
+    };
+    const int rc = alloc();
+    if (rc != B200LDU_OK) {
+        b200ldu_matrix_destroy(m);
+        return rc;
+    }
     *out = m;
     return B200LDU_OK;
 }
@@ -333,14 +315,7 @@ extern "C" int b200ldu_matrix_destroy(b200ldu_matrix *m)
     if (!m) return B200LDU_OK;
     cudaSetDevice(m->a->ctx->device);
     cudaStreamSynchronize(m->a->ctx->stream);
-    if (m->d_valT && m->d_valT != m->d_val) cudaFree(m->d_valT);
-    void *ptrs[] = {m->d_val, m->d_fval, m->d_diag, m->d_rD, m->d_partials, m->d_scal, m->d_hist, m->d_sendBuf,
-                    m->own[0], m->own[1], m->own[2], m->own[3], m->own[4]};
-    for (void *p : ptrs)
-        if (p) cudaFree(p);
-    for (double *p : m->work)
-        if (p) cudaFree(p);
-    delete m;
+    delete m; // its DeviceMem frees every device array
     return B200LDU_OK;
 }
 
@@ -383,21 +358,20 @@ __global__ void fill_diag_kernel(long long n, int nPad, const int *__restrict__ 
     rD[r] = __ddiv_rn(1.0, d); // AINVPreconditioner.C:34-41, diagonalPreconditioner.C:60-66
 }
 
-// caller-order copy kept by the matrix (slot k of m->own), grown on demand
+// caller-order copy kept by the matrix in slot k; a copy the matrix stops using is released.  The caller may pass
+// back the matrix's own array (src is then the slot itself and nothing is copied).
 static int own_copy(b200ldu_matrix *m, int k, const double *src, size_t n, const double **out)
 {
     *out = nullptr;
-    if (!src || n == 0) return B200LDU_OK;
-    if (m->ownLen[k] < n) {
-        if (m->own[k]) cudaFree(m->own[k]);
-        m->own[k] = nullptr;
-        m->ownLen[k] = 0;
-        CUDA_TRY(cudaMalloc((void **)&m->own[k], sizeof(double) * n));
-        m->ownLen[k] = n;
+    if (!src || n == 0) {
+        m->mem.release(k);
+        return B200LDU_OK;
     }
-    if (src != m->own[k])
-        CUDA_TRY(cudaMemcpyAsync(m->own[k], src, sizeof(double) * n, cudaMemcpyDeviceToDevice, m->a->ctx->stream));
-    *out = m->own[k];
+    double *own = nullptr;
+    TRY(m->mem.slot(k, own, n));
+    if (src != own)
+        CUDA_TRY(cudaMemcpyAsync(own, src, sizeof(double) * n, cudaMemcpyDeviceToDevice, m->a->ctx->stream));
+    *out = own;
     return B200LDU_OK;
 }
 
@@ -434,38 +408,38 @@ extern "C" int b200ldu_matrix_set(b200ldu_matrix *m, const double *diag_d, const
     // lduMatrix.C:202-218): faceH, the fvMatrix glue and the GAMG coarse-level assembly read them
     // later, so the caller may free or overwrite its arrays as soon as this call returns.
     const double *dg, *up, *lw, *bo, *in;
-    TRY(own_copy(m, 0, diag_d, (size_t)a->nCells, &dg));
-    TRY(own_copy(m, 1, upper_d, (size_t)a->nFaces, &up));
-    TRY(own_copy(m, 2, lower_d, (size_t)a->nFaces, &lw));
-    TRY(own_copy(m, 3, bou_d, (size_t)a->L.nRecv, &bo));
-    if (sameIfc)
-        in = bo;
-    else
-        TRY(own_copy(m, 4, int_d, (size_t)a->L.nRecv, &in));
+    TRY(own_copy(m, MAT_OWN_DIAG, diag_d, (size_t)a->nCells, &dg));
+    TRY(own_copy(m, MAT_OWN_UPPER, upper_d, (size_t)a->nFaces, &up));
+    TRY(own_copy(m, MAT_OWN_LOWER, lower_d, (size_t)a->nFaces, &lw));
+    TRY(own_copy(m, MAT_OWN_BOU, bou_d, (size_t)a->L.nRecv, &bo));
+    TRY(own_copy(m, MAT_OWN_INT, sameIfc ? nullptr : int_d, (size_t)a->L.nRecv, &in));
+    if (sameIfc) in = bo;
     const double *lo = lw ? lw : up;
     long long ne = a->nEntries;
     // Tmul needs its own coefficient stream when A != A^T (asymmetric coefficients or
     // interfaceIntCoeffs != interfaceBouCoeffs)
     bool needT = !m->symmetric || (a->L.nRecv && !sameIfc);
+    // the stream a matrix stops using is released: at 256^3 either one is about 0.8 GB
     if (!needT && a->hasFs) {
         // A == A^T: the face stream holds every face once and serves both
-        if (m->d_valT && m->d_valT != m->d_val) cudaFree(m->d_valT);
-        if (m->d_val) cudaFree(m->d_val);
+        m->mem.release(MAT_VAL);
+        m->mem.release(MAT_VALT);
         m->d_val = m->d_valT = nullptr;
         const long long nf = a->fsOwn + a->fsList;
-        if (!m->d_fval) CUDA_TRY(cudaMalloc((void **)&m->d_fval, sizeof(double) * (size_t)(nf > 0 ? nf : 1)));
+        TRY(m->mem.slot(MAT_FVAL, m->d_fval, (size_t)nf));
         if (nf > 0) {
             fill_val_kernel<<<(unsigned)((nf + 255) / 256), 256, 0, st>>>(nf, a->d_fsCode, up, lo, bo, m->d_fval, 0);
             a->ctx->launches++;
         }
     } else {
-        if (m->d_fval) cudaFree(m->d_fval);
+        m->mem.release(MAT_FVAL);
         m->d_fval = nullptr;
-        size_t nb = sizeof(double) * (size_t)(ne > 0 ? ne : 1);
-        if (!m->d_val) CUDA_TRY(cudaMalloc((void **)&m->d_val, nb));
-        if (needT && (!m->d_valT || m->d_valT == m->d_val)) {
-            m->d_valT = nullptr;
-            CUDA_TRY(cudaMalloc((void **)&m->d_valT, nb));
+        TRY(m->mem.slot(MAT_VAL, m->d_val, (size_t)ne));
+        if (needT)
+            TRY(m->mem.slot(MAT_VALT, m->d_valT, (size_t)ne));
+        else {
+            m->mem.release(MAT_VALT);
+            m->d_valT = m->d_val; // A^T == A
         }
         if (ne > 0) {
             unsigned g = (unsigned)((ne + 255) / 256);
@@ -475,10 +449,6 @@ extern "C" int b200ldu_matrix_set(b200ldu_matrix *m, const double *diag_d, const
                 fill_val_kernel<<<g, 256, 0, st>>>(ne, a->d_code, up, lo, in, m->d_valT, 1);
                 a->ctx->launches++;
             }
-        }
-        if (!needT) {
-            if (m->d_valT && m->d_valT != m->d_val) cudaFree(m->d_valT);
-            m->d_valT = m->d_val; // A^T == A
         }
     }
     KERNEL_CHECK();
@@ -625,7 +595,7 @@ static int amul_ext(b200ldu_matrix *m, bool T, const double *psi, double *out)
     CHECK_M(m);
     if (!psi || !out) return B200LDU_EINVAL;
     b200ldu_addr *a = m->a;
-    double *xb = addr_pool_vec(a, 0), *yb = addr_pool_vec(a, 1);
+    double *xb = banded_vec(a, a->mem, ADDR_X), *yb = banded_vec(a, a->mem, ADDR_Y);
     if (!xb || !yb) return B200LDU_ECUDA;
     TRY(to_banded(a, psi, xb));
     TRY(mat_amul(m, T, xb, yb, 0, nullptr, nullptr, nullptr));
@@ -651,7 +621,7 @@ extern "C" int b200ldu_amul_banded(b200ldu_matrix *m, const double *psib_d, doub
 extern "C" int b200ldu_sumA(b200ldu_matrix *m, double *sumA_d)
 {
     CHECK_M(m);
-    double *yb = addr_pool_vec(m->a, 1);
+    double *yb = banded_vec(m->a, m->a->mem, ADDR_Y);
     if (!yb) return B200LDU_ECUDA;
     TRY(mat_sumA(m, yb, nullptr));
     return from_banded(m->a, yb, sumA_d);
@@ -662,7 +632,7 @@ extern "C" int b200ldu_residual(b200ldu_matrix *m, const double *psi_d, const do
 {
     CHECK_M(m);
     b200ldu_addr *a = m->a;
-    double *xb = addr_pool_vec(a, 0), *yb = addr_pool_vec(a, 1), *bb = addr_pool_vec(a, 2);
+    double *xb = banded_vec(a, a->mem, ADDR_X), *yb = banded_vec(a, a->mem, ADDR_Y), *bb = banded_vec(a, a->mem, ADDR_B);
     if (!xb || !yb || !bb) return B200LDU_ECUDA;
     TRY(to_banded(a, psi_d, xb));
     TRY(to_banded(a, source_d, bb));
@@ -674,7 +644,7 @@ extern "C" int b200ldu_H(b200ldu_matrix *m, const double *psi_d, double *Hpsi_d)
 {
     CHECK_M(m);
     b200ldu_addr *a = m->a;
-    double *xb = addr_pool_vec(a, 0), *yb = addr_pool_vec(a, 1);
+    double *xb = banded_vec(a, a->mem, ADDR_X), *yb = banded_vec(a, a->mem, ADDR_Y);
     if (!xb || !yb) return B200LDU_ECUDA;
     TRY(to_banded(a, psi_d, xb));
     TRY(mat_H(m, xb, yb));
@@ -684,7 +654,7 @@ extern "C" int b200ldu_H(b200ldu_matrix *m, const double *psi_d, double *Hpsi_d)
 extern "C" int b200ldu_H1(b200ldu_matrix *m, double *H1_d)
 {
     CHECK_M(m);
-    double *yb = addr_pool_vec(m->a, 1);
+    double *yb = banded_vec(m->a, m->a->mem, ADDR_Y);
     if (!yb) return B200LDU_ECUDA;
     TRY(mat_H1(m, yb));
     return from_banded(m->a, yb, H1_d);
@@ -783,7 +753,7 @@ extern "C" int b200ldu_precondition(b200ldu_matrix *m, const char *name, int tra
     int k = precond_kind(name, printed);
     if (k < 0) return B200LDU_ENOPRECOND;
     b200ldu_addr *a = m->a;
-    double *xb = addr_pool_vec(a, 0), *yb = addr_pool_vec(a, 1);
+    double *xb = banded_vec(a, a->mem, ADDR_X), *yb = banded_vec(a, a->mem, ADDR_Y);
     if (!xb || !yb) return B200LDU_ECUDA;
     TRY(to_banded(a, rA_d, xb));
     TRY(mat_precondition(m, k, transpose != 0, xb, yb, false, nullptr, nullptr, nullptr, nullptr));
@@ -804,7 +774,7 @@ extern "C" int b200ldu_smooth(b200ldu_matrix *m, const char *name, double omega,
     CHECK_M(m);
     if (!smoother_ok(name)) return B200LDU_ENOPRECOND;
     b200ldu_addr *a = m->a;
-    double *xb = addr_pool_vec(a, 0), *yb = addr_pool_vec(a, 1), *bb = addr_pool_vec(a, 2);
+    double *xb = banded_vec(a, a->mem, ADDR_X), *yb = banded_vec(a, a->mem, ADDR_Y), *bb = banded_vec(a, a->mem, ADDR_B);
     if (!xb || !yb || !bb) return B200LDU_ECUDA;
     TRY(to_banded(a, psi_d, xb));
     TRY(to_banded(a, source_d, bb));

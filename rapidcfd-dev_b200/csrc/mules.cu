@@ -32,16 +32,10 @@ static int mules_limiter_impl(int corr, double extrema, b200ldu_addr *a, int nLi
     cudaStream_t st = ctx->stream;
     const int n = a->nCells, nF = a->nFaces, nB = a->nBFaces;
     // scratch: psiMaxn, psiMinn, sumPhip, mSumPhim, lambdam, lambdap (six cell fields, kept across calls) + the received limiters
-    const size_t need = (size_t)6 * n + (size_t)nCoupledFaces;
-    if (a->mulesScratchLen < need) {
-        if (a->d_mulesScratch) cudaFree(a->d_mulesScratch);
-        a->d_mulesScratch = nullptr;
-        a->mulesScratchLen = 0;
-        CUDA_TRY(cudaMalloc((void **)&a->d_mulesScratch, sizeof(double) * need));
-        a->mulesScratchLen = need;
-    }
-    double *psiMaxn = a->d_mulesScratch, *psiMinn = psiMaxn + n, *sumPhip = psiMinn + n, *mSumPhim = sumPhip + n,
-           *lambdam = mSumPhim + n, *lambdap = lambdam + n, *theirs = lambdap + n;
+    double *psiMaxn = nullptr;
+    TRY(a->mem.slot(ADDR_MULES, psiMaxn, (size_t)6 * n + (size_t)nCoupledFaces));
+    double *psiMinn = psiMaxn + n, *sumPhip = psiMinn + n, *mSumPhim = sumPhip + n, *lambdam = mSumPhim + n,
+           *lambdap = lambdam + n, *theirs = lambdap + n;
     const int *bs = nB ? a->d_bCellStart : nullptr;
     // lambda_d / lambdaB_d come in holding the starting limiter (MULES::limit: allLambda(mesh.nFaces(), 1.0))
     mules_bounds_kernel<<<(n + 127) / 128, 128, 0, st>>>(n, a->d_ownerStart, a->d_u, a->d_losortStart, a->d_losort, a->d_l, bs,

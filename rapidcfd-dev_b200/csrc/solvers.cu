@@ -522,11 +522,7 @@ int solve_diagonal(Solve &S)
 
 double *Solve::vec(int k)
 {
-    while ((int)m->work.size() <= k) m->work.push_back(nullptr);
-    if (!m->work[k]) {
-        if (addr_alloc_vec(m->a, &m->work[k]) != B200LDU_OK) return nullptr;
-    }
-    return m->work[k];
+    return k < MAT_NWORK ? banded_vec(m->a, m->mem, MAT_WORK + k) : nullptr;
 }
 
 int gamg_solve(Solve &S, b200ldu_gamg *g, const char *smoother); // gamg.cu
@@ -553,15 +549,7 @@ int solve_banded(b200ldu_matrix *m, const char *solver, const char *pre, const b
     *resultBuf = psi_b;
 
     // residual history buffer on the device
-    if (histCap > 0 && hist_h) {
-        if (m->histCap < histCap) {
-            if (m->d_hist) cudaFree(m->d_hist);
-            m->d_hist = nullptr;
-            CUDA_TRY(cudaMalloc((void **)&m->d_hist, sizeof(double) * (size_t)histCap));
-            m->histCap = histCap;
-        }
-        S.hist = m->d_hist;
-    }
+    if (histCap > 0 && hist_h) TRY(m->mem.slot(MAT_HIST, S.hist, (size_t)histCap));
     // pinned flags + events
     void *pin = nullptr;
     TRY(ctx_pinned(ctx, 4096, &pin));
@@ -728,7 +716,7 @@ int solve_banded(b200ldu_matrix *m, const char *solver, const char *pre, const b
             if (!strcmp(perf->solverName, "smoothSolver") && S.c.nSweeps > 0) k = perf->nIterations / S.c.nSweeps + 1;
             if (k > histCap) k = histCap;
             if (S.noScalars || S.fixedSweeps) k = 0;
-            if (k > 0) CUDA_TRY(cudaMemcpy(hist_h, m->d_hist, sizeof(double) * (size_t)k, cudaMemcpyDeviceToHost));
+            if (k > 0) CUDA_TRY(cudaMemcpy(hist_h, S.hist, sizeof(double) * (size_t)k, cudaMemcpyDeviceToHost));
             for (int i = k; i < histCap; i++) hist_h[i] = NAN;
         }
     } else {
@@ -749,10 +737,8 @@ extern "C" int b200ldu_solve(b200ldu_matrix *m, const char *solver, const char *
     }
     CUDA_TRY(cudaSetDevice(m->a->ctx->device));
     b200ldu_addr *a = m->a;
-    // banded copies of psi and source live with the matrix workspace (slots 14, 15)
-    Solve tmp;
-    tmp.m = m;
-    double *psi_b = tmp.vec(14), *src_b = tmp.vec(15);
+    // banded copies of psi and source live with the matrix workspace
+    double *psi_b = banded_vec(a, m->mem, MAT_PSI), *src_b = banded_vec(a, m->mem, MAT_SRC);
     if (!psi_b || !src_b) return B200LDU_ECUDA;
     TRY(to_banded(a, psi_d, psi_b));
     TRY(to_banded(a, source_d, src_b));
@@ -775,9 +761,7 @@ extern "C" int b200ldu_solve_host(b200ldu_matrix *m, const char *solver, const c
     b200ldu_ctx *ctx = a->ctx;
     CUDA_TRY(cudaSetDevice(ctx->device));
     size_t bytes = sizeof(double) * (size_t)a->nCells;
-    Solve tmp;
-    tmp.m = m;
-    double *psi_d = tmp.vec(12), *src_d = tmp.vec(13);
+    double *psi_d = banded_vec(a, m->mem, MAT_HOST_PSI), *src_d = banded_vec(a, m->mem, MAT_HOST_SRC);
     if (!psi_d || !src_d) return B200LDU_ECUDA;
     // host buffers may be pageable: cudaMemcpyAsync then stages through the driver's pinned pool
     CUDA_TRY(cudaMemcpyAsync(psi_d, psi_h, bytes, cudaMemcpyHostToDevice, ctx->stream));
