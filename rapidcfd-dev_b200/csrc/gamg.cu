@@ -715,7 +715,7 @@ int smooth_in_place(Solve &S, b200ldu_matrix *m, double omega, double *&x, doubl
 int gamg_scale(Solve &S, b200ldu_matrix *m, double *field, double *Acf, const double *source, const int *stop)
 {
     SolverScalars *sc = S.sc;
-    TRY(mat_amul(m, false, field, Acf, 2, source, m->d_partials, stop));
+    TRY(mat_amul(m, false, field, Acf, AMUL_AUX_X_OUT_X, source, m->d_partials, stop));
     TRY(scalar_step_on<2>(S, m->d_partials, m->a->L.nBands, [=] __device__(SolverScalars *s) {
         double den = s->sum[1];
         double sden = den >= 0 ? den + VSMALL_ : den - VSMALL_; // stabilise(y, VSMALL)
@@ -874,9 +874,8 @@ static int gamg_cycle(Solve &S, b200ldu_gamg *g, int scaleCorrection, double *co
                       double *&Apsi, double *&finestCorr, double *finestRes)
 {
     const b200ldu_controls &c = S.c;
-    SolverScalars *sc = S.sc;
     double *hist = S.hist;
-    const int *stop = &sc->stop;
+    const int *stop = S.stop;
     cudaStream_t st = S.ctx->stream;
     b200ldu_matrix *fm = S.m;
     const int nL = g->nLevels, coarsest = nL - 1;
@@ -895,7 +894,7 @@ static int gamg_cycle(Solve &S, b200ldu_gamg *g, int scaleCorrection, double *co
             TRY(smooth_in_place(S, L.mat, omega, L.corr, L.tmp, L.src,
                                 imin(c.nPreSweeps + c.preSweepsLevelMultiplier * k, c.maxPreSweeps), stop));
             if (scaleCorrection && k < coarsest - 1) TRY(gamg_scale(S, L.mat, L.corr, L.acf, L.src, stop));
-            TRY(mat_amul(L.mat, false, L.corr, L.acf, 0, nullptr, nullptr, stop));
+            TRY(mat_amul(L.mat, false, L.corr, L.acf, AMUL_ONLY, nullptr, nullptr, stop));
             double *src = L.src, *acf = L.acf;
             TRY(ew_launch<0>(S.ctx, L.addr->L.nPad / 2, stop, nullptr, nullptr, [=] __device__(int i, double *) {
                 double2 s2 = CV2(src)[i], a2 = CV2(acf)[i];
@@ -1008,7 +1007,7 @@ static int gamg_cycle(Solve &S, b200ldu_gamg *g, int scaleCorrection, double *co
     TRY(smooth_in_place(S, fm, omega, psi, spare, S.src, nFinest, stop));
     finestSweeps += nFinest;
     // ---- finest residual + convergence (:146-175) ----
-    TRY(mat_amul(fm, false, psi, Apsi, 0, nullptr, nullptr, stop));
+    TRY(mat_amul(fm, false, psi, Apsi, AMUL_ONLY, nullptr, nullptr, stop));
     int np = 0;
     {
         const double *b = S.src, *Ap = Apsi;
@@ -1031,9 +1030,9 @@ static int gamg_cycle(Solve &S, b200ldu_gamg *g, int scaleCorrection, double *co
     return B200LDU_OK;
 }
 
-int gamg_solve(Solve &S, b200ldu_gamg *g, const char *smoother)
+// the smoother was checked by the selection (solvers.cu): Jacobi is the only one (GaussSeidel aliases to it)
+int gamg_solve(Solve &S, b200ldu_gamg *g)
 {
-    (void)smoother; // validated by the caller; Jacobi is the only smoother (GaussSeidel aliases to it)
     if (!g || g->nLevels == 0) {
         b200_set_error("GAMG: No coarse levels created, either matrix too small for GAMG or "
                        "nCellsInCoarsestLevel too large (GAMGSolver.C:174-192)");
@@ -1048,6 +1047,8 @@ int gamg_solve(Solve &S, b200ldu_gamg *g, const char *smoother)
     double *const psiBuf[2] = {S.psi, S.vec(0)};
     double *Apsi = S.vec(1), *finestCorr = S.vec(2), *finestRes = S.vec(3);
     if (!psiBuf[1] || !Apsi || !finestCorr || !finestRes) return B200LDU_ECUDA;
+    // psi ping-pongs between psiBuf[0] and [1] with the finest sweeps of each cycle
+    S.result = SolveResult{{psiBuf[0], psiBuf[1]}, S.c.nFinestSweeps > 0 ? S.c.nFinestSweeps : 0, 1};
 
     TRY(gamg_build_matrices(S, g));
     if (S.c.directSolveCoarsest) {
@@ -1056,18 +1057,14 @@ int gamg_solve(Solve &S, b200ldu_gamg *g, const char *smoother)
         S.useGraph = false; // the coarsest-level Krylov solve synchronises with the host
         S.c.checkEvery = 1;
     }
-    TRY(mat_amul(fm, false, S.psi, Apsi, 0, nullptr, nullptr, nullptr));
+    TRY(mat_amul(fm, false, S.psi, Apsi, AMUL_ONLY, nullptr, nullptr, nullptr));
     TRY(init_residual(S, S.psi, S.src, Apsi, finestRes, finestCorr));
     long long maxBodies = S.c.maxIter > S.c.minIter ? S.c.maxIter : S.c.minIter;
     if (maxBodies < 1) maxBodies = 1;
     // counted when a cycle is enqueued, so not on graph replays: a captured chunk has an even number of cycles, which
     // brings the parity back to the buffers the capture started from
     long long finestSweeps = 0;
-    TRY(run_iterations(S, maxBodies, [&](long long) {
+    return run_iterations(S, maxBodies, [&](long long) {
         return gamg_cycle(S, g, scaleCorrection, psiBuf, finestSweeps, Apsi, finestCorr, finestRes);
-    }));
-    S.smoothBuf[0] = psiBuf[0];
-    S.smoothBuf[1] = psiBuf[1];
-    S.sweepsPerIteration = S.c.nFinestSweeps > 0 ? S.c.nFinestSweeps : 0;
-    return B200LDU_OK;
+    });
 }

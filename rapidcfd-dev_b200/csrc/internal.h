@@ -53,9 +53,7 @@ struct b200ldu_ctx {
     // NCCL (comm.cu)
     void *nccl = nullptr; // ncclComm_t
     int rank = 0, nRanks = 1;
-    // pinned staging for *_host entry points and scalar read-back
-    void *pinned = nullptr;
-    size_t pinnedBytes = 0;
+    struct PinnedArea *pinned = nullptr; // page-locked: the solvers' stop flags and scalar read-back (ops.cuh)
     // peer-memory (CUDA IPC over NVLink) collectives, see comm.cu
     bool p2p = false;
     char *region = nullptr;          // this rank's shared region

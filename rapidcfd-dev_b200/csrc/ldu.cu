@@ -72,8 +72,7 @@ extern "C" int b200ldu_ctx_create(int device, b200ldu_ctx **out)
     c->smCount = p.multiProcessorCount;
     CUDA_TRY(cudaStreamCreateWithFlags(&c->ownStream, cudaStreamNonBlocking));
     c->stream = c->ownStream;
-    c->pinnedBytes = 1 << 16;
-    CUDA_TRY(cudaMallocHost(&c->pinned, c->pinnedBytes));
+    CUDA_TRY(cudaMallocHost(&c->pinned, sizeof(PinnedArea)));
     *out = c;
     return B200LDU_OK;
 }
@@ -110,19 +109,6 @@ extern "C" int b200ldu_ctx_device_mem(const b200ldu_ctx *c, long long *liveBytes
     if (!c) return B200LDU_EINVAL;
     if (liveBytes) *liveBytes = c->memLive;
     if (nAllocs) *nAllocs = c->memAllocs;
-    return B200LDU_OK;
-}
-
-int ctx_pinned(b200ldu_ctx *c, size_t bytes, void **out)
-{
-    if (bytes > c->pinnedBytes) {
-        if (c->pinned) cudaFreeHost(c->pinned);
-        c->pinned = nullptr;
-        c->pinnedBytes = 0;
-        CUDA_TRY(cudaMallocHost(&c->pinned, bytes));
-        c->pinnedBytes = bytes;
-    }
-    *out = c->pinned;
     return B200LDU_OK;
 }
 
@@ -468,7 +454,7 @@ int mat_halo(b200ldu_matrix *m, double *x, const int *stop, int *usedP2P)
     return comm_halo_exchange(m->a, x, m->d_sendBuf, stop, usedP2P);
 }
 
-int mat_amul(b200ldu_matrix *m, bool transpose, double *x, double *out, int mode, const double *aux,
+int mat_amul(b200ldu_matrix *m, bool transpose, double *x, double *out, AmulSum sum, const double *aux,
              double *partials, const int *stop)
 {
     int wait = 0;
@@ -483,12 +469,12 @@ int mat_amul(b200ldu_matrix *m, bool transpose, double *x, double *out, int mode
         op.out = out;
         return engine_launch_m(m, transpose, op);
     };
-    switch (mode) {
-    case 0: return launch(AmulOp<0>());
-    case 1: return launch(AmulOp<1>());
-    case 2: return launch(AmulOp<2>());
-    case 3: return launch(AmulOp<3>());
-    case 4: return launch(AmulOp<4>());
+    switch (sum) {
+    case AMUL_ONLY: return launch(AmulOp<AMUL_ONLY>());
+    case AMUL_OUT_X: return launch(AmulOp<AMUL_OUT_X>());
+    case AMUL_AUX_X_OUT_X: return launch(AmulOp<AMUL_AUX_X_OUT_X>());
+    case AMUL_OUT_AUX: return launch(AmulOp<AMUL_OUT_AUX>());
+    case AMUL_OUT_OUT_OUT_AUX: return launch(AmulOp<AMUL_OUT_OUT_OUT_AUX>());
     }
     return B200LDU_EINVAL;
 }
@@ -598,7 +584,7 @@ static int amul_ext(b200ldu_matrix *m, bool T, const double *psi, double *out)
     double *xb = banded_vec(a, a->mem, ADDR_X), *yb = banded_vec(a, a->mem, ADDR_Y);
     if (!xb || !yb) return B200LDU_ECUDA;
     TRY(to_banded(a, psi, xb));
-    TRY(mat_amul(m, T, xb, yb, 0, nullptr, nullptr, nullptr));
+    TRY(mat_amul(m, T, xb, yb, AMUL_ONLY, nullptr, nullptr, nullptr));
     return from_banded(a, yb, out);
 }
 
@@ -615,7 +601,7 @@ extern "C" int b200ldu_tmul(b200ldu_matrix *m, const double *psi_d, double *Tpsi
 extern "C" int b200ldu_amul_banded(b200ldu_matrix *m, const double *psib_d, double *Apsib_d)
 {
     CHECK_M(m);
-    return mat_amul(m, false, const_cast<double *>(psib_d), Apsib_d, 0, nullptr, nullptr, nullptr);
+    return mat_amul(m, false, const_cast<double *>(psib_d), Apsib_d, AMUL_ONLY, nullptr, nullptr, nullptr);
 }
 
 extern "C" int b200ldu_sumA(b200ldu_matrix *m, double *sumA_d)
@@ -794,9 +780,9 @@ extern "C" int b200ldu_bench_op(b200ldu_matrix *m, const char *op, double *xb, d
 {
     CHECK_M(m);
     if (!op || !xb || !yb) return B200LDU_EINVAL;
-    if (!strcmp(op, "amul")) return mat_amul(m, false, xb, yb, 0, nullptr, nullptr, nullptr);
-    if (!strcmp(op, "tmul")) return mat_amul(m, true, xb, yb, 0, nullptr, nullptr, nullptr);
-    if (!strcmp(op, "amul_dot")) return mat_amul(m, false, xb, yb, 1, nullptr, m->d_partials, nullptr);
+    if (!strcmp(op, "amul")) return mat_amul(m, false, xb, yb, AMUL_ONLY, nullptr, nullptr, nullptr);
+    if (!strcmp(op, "tmul")) return mat_amul(m, true, xb, yb, AMUL_ONLY, nullptr, nullptr, nullptr);
+    if (!strcmp(op, "amul_dot")) return mat_amul(m, false, xb, yb, AMUL_OUT_X, nullptr, m->d_partials, nullptr);
     if (!strcmp(op, "ainv")) return mat_ainv(m, false, xb, yb, false, nullptr, nullptr, nullptr);
     if (!strcmp(op, "ainv_dot")) return mat_ainv(m, false, xb, yb, true, nullptr, m->d_partials, nullptr);
     if (!strcmp(op, "jacobi")) return bb ? mat_jacobi(m, 0.9, xb, bb, yb, nullptr) : B200LDU_EINVAL;

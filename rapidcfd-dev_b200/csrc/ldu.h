@@ -2,13 +2,19 @@
 #pragma once
 #include "internal.h"
 
-int ctx_pinned(b200ldu_ctx *c, size_t bytes, void **out);
 int matrix_set_diag(b200ldu_matrix *m, const double *diag_d); // banded diag + 1/diag; re-points diag_ext
 int to_banded(b200ldu_addr *a, const double *x, double *xb);
 int from_banded(b200ldu_addr *a, const double *xb, double *x);
 int mat_halo(b200ldu_matrix *m, double *x, const int *stop, int *usedP2P);
-// mode: see AmulOp in ops.cuh
-int mat_amul(b200ldu_matrix *m, bool transpose, double *x, double *out, int mode, const double *aux,
+// what an Amul sweep sums into its partials besides out = A x
+enum AmulSum {
+    AMUL_ONLY,            // nothing
+    AMUL_OUT_X,           // <out,x>: PCG wApA
+    AMUL_AUX_X_OUT_X,     // <aux,x>, <out,x>: GAMG scale num = <source,field>, den = <Acf,field> (GAMGSolverScale.C:80-125)
+    AMUL_OUT_AUX,         // <out,aux>: PBiCG wApT, PBiCGStab rA0AyA
+    AMUL_OUT_OUT_OUT_AUX, // <out,out>, <out,aux>: PBiCGStab tAtA, tAsA
+};
+int mat_amul(b200ldu_matrix *m, bool transpose, double *x, double *out, AmulSum sum, const double *aux,
              double *partials, const int *stop);
 int mat_ainv(b200ldu_matrix *m, bool transpose, const double *r, double *w, bool fuseDot,
              const double *dotv, double *partials, const int *stop);

@@ -2,6 +2,7 @@
 // kernels used by the solvers.  See engine.cuh for the Op concept.
 #pragma once
 #include "engine.cuh"
+#include "ldu.h"
 
 // device-resident solver state: alpha/beta and the convergence decision never leave
 // the GPU inside the iteration loop (the reference synchronises the host three times
@@ -21,6 +22,15 @@ struct SolverScalars {
     // that the waiting CTAs' polling does not slow down CTA 0's writes to the scalars above.
     alignas(128) unsigned long long gate;
     unsigned long long gatePad[15];
+};
+
+// Page-locked host area of a context (b200ldu_ctx::pinned), allocated once with the context and never moved: a
+// nested solve must not free what the outer solve is still polling.
+constexpr int SOLVE_MAX_DEPTH = 8; // GAMG nests one Krylov solve; deeper nesting is refused
+struct PinnedArea {
+    int flags[SOLVE_MAX_DEPTH][2]; // stop-flag pair polled by the solve at each nesting depth (run_iterations)
+    SolverScalars scalars;         // read back at the end of a solve
+    unsigned long long peerErr;    // a bounded wait on a peer's flag gave up (engine.cuh spin_until)
 };
 
 struct OpBase {
@@ -49,13 +59,10 @@ struct StageXOp : OpBase {
     }
 };
 
-// ---- Amul / Tmul: out = diag*x + sum v*x[c]  (lduMatrixATmul.C:78-137) ----
-// MODE 0 plain; 1: sum(out*x) [PCG wApA];  2: sum(aux*x), sum(out*x) [GAMG scale: num =
-// <source,field>, den = <Acf,field>, GAMGSolverScale.C:80-125];  3: sum(out*aux) [PBiCG
-// wApT, PBiCGStab rA0AyA];  4: sum(out*out), sum(out*aux) [PBiCGStab tAtA, tAsA]
-template <int MODE>
+// ---- Amul / Tmul: out = diag*x + sum v*x[c]  (lduMatrixATmul.C:78-137), with the sums of AmulSum (ldu.h) ----
+template <AmulSum MODE>
 struct AmulOp : StageXOp {
-    static constexpr int NRED = (MODE == 0) ? 0 : ((MODE == 1 || MODE == 3) ? 1 : 2);
+    static constexpr int NRED = MODE == AMUL_ONLY ? 0 : ((MODE == AMUL_OUT_X || MODE == AMUL_OUT_AUX) ? 1 : 2);
     static constexpr bool LOCAL = false;
     const double *diag, *aux;
     double *out;
@@ -63,13 +70,13 @@ struct AmulOp : StageXOp {
     __device__ __forceinline__ void finish(int r, double acc0, double acc1, double a0, double a1, double *red) const
     {
         *reinterpret_cast<double2 *>(out + r) = make_double2(acc0, acc1);
-        if (MODE == 1) red[0] += acc0 * a0 + acc1 * a1;
-        if (MODE == 2) {
+        if (MODE == AMUL_OUT_X) red[0] += acc0 * a0 + acc1 * a1;
+        if (MODE == AMUL_AUX_X_OUT_X) {
             red[0] += aux[r] * a0 + aux[r + 1] * a1;
             red[1] += acc0 * a0 + acc1 * a1;
         }
-        if (MODE == 3) red[0] += acc0 * aux[r] + acc1 * aux[r + 1];
-        if (MODE == 4) {
+        if (MODE == AMUL_OUT_AUX) red[0] += acc0 * aux[r] + acc1 * aux[r + 1];
+        if (MODE == AMUL_OUT_OUT_OUT_AUX) {
             red[0] += acc0 * acc0 + acc1 * acc1;
             red[1] += acc0 * aux[r] + acc1 * aux[r + 1];
         }
@@ -196,10 +203,17 @@ struct OffDiagOp : StageXOp {
 // ---------------------------------------------------------------------------
 constexpr int EW_THREADS = 256;
 
-template <int NRED, class F>
-__global__ void __launch_bounds__(EW_THREADS) ew_kernel(int n2, const int *stop, double *partials, F f)
+// prologue of an element-wise kernel that has no deferred scalar step to run
+struct NoPrologue {
+    __device__ __forceinline__ bool run() const { return true; }
+};
+
+// pre.run() first: a deferred scalar step (DeferredStep below) or nothing
+template <int NRED, class F, class Pre>
+__global__ void __launch_bounds__(EW_THREADS) ew_kernel(int n2, const int *stop, double *partials, F f, Pre pre)
 {
     if (stop && *stop) return;
+    if (!pre.run()) return;
     double red[NRED > 0 ? NRED : 1];
 #pragma unroll
     for (int k = 0; k < (NRED > 0 ? NRED : 1); k++) red[k] = 0;
@@ -214,35 +228,11 @@ inline int ew_grid(const b200ldu_ctx *ctx, int n2)
     return want < 1 ? 1 : (want < cap ? want : cap);
 }
 
-template <int NRED, class F>
-int ew_launch(b200ldu_ctx *ctx, int n2, const int *stop, double *partials, int *nPartialsOut, F f)
+template <int NRED, class F, class Pre = NoPrologue>
+int ew_launch(b200ldu_ctx *ctx, int n2, const int *stop, double *partials, int *nPartialsOut, F f, Pre pre = Pre())
 {
     int g = ew_grid(ctx, n2);
-    ew_kernel<NRED, F><<<g, EW_THREADS, 0, ctx->stream>>>(n2, stop, partials, f);
-    ctx->launches++;
-    if (nPartialsOut) *nPartialsOut = g;
-    KERNEL_CHECK();
-    return B200LDU_OK;
-}
-
-// element-wise kernel that first runs a deferred scalar step (DeferredStep below) in its prologue
-template <int NRED, class F, class Pre>
-__global__ void __launch_bounds__(EW_THREADS) ew_kernel_pre(int n2, const int *stop, double *partials, F f, Pre pre)
-{
-    if (stop && *stop) return;
-    if (!pre.run()) return;
-    double red[NRED > 0 ? NRED : 1];
-#pragma unroll
-    for (int k = 0; k < (NRED > 0 ? NRED : 1); k++) red[k] = 0;
-    for (int i = blockIdx.x * EW_THREADS + threadIdx.x; i < n2; i += gridDim.x * EW_THREADS) f(i, red);
-    if (NRED > 0) block_reduce_store<(NRED > 0 ? NRED : 1), EW_THREADS>(red, partials, blockIdx.x);
-}
-
-template <int NRED, class F, class Pre>
-int ew_launch(b200ldu_ctx *ctx, int n2, const int *stop, double *partials, int *nPartialsOut, F f, Pre pre)
-{
-    int g = ew_grid(ctx, n2);
-    ew_kernel_pre<NRED, F, Pre><<<g, EW_THREADS, 0, ctx->stream>>>(n2, stop, partials, f, pre);
+    ew_kernel<NRED, F, Pre><<<g, EW_THREADS, 0, ctx->stream>>>(n2, stop, partials, f, pre);
     ctx->launches++;
     if (nPartialsOut) *nPartialsOut = g;
     KERNEL_CHECK();
@@ -439,10 +429,10 @@ struct PcgAinvOp : OpBase {
 // K_B: applies the solution update of the PREVIOUS body (psi += alpha pOld, own rows, in
 // place) and forms the new search direction while staging (p = z on the first body, else
 // z + beta p; alpha, beta from the device scalars; p ping-ponged), then the row arithmetic
-// of AmulOp<1>: w = A p, fused <w,p>.  The halo send (fused pack CTAs) stages the same p at
+// of AmulOp<AMUL_OUT_X>: w = A p, fused <w,p>.  The halo send (fused pack CTAs) stages the same p at
 // the patch face cells: stage() stays free of psi.
 template <class Pre>
-struct PcgAmulOp : AmulOp<1> {
+struct PcgAmulOp : AmulOp<AMUL_OUT_X> {
     const double *z, *pOld;
     double *pNew, *psi;
     const SolverScalars *sc;

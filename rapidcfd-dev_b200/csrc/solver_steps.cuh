@@ -4,6 +4,8 @@
 #include "ops.cuh"
 #include "solvers.h"
 
+#include <algorithm>
+
 static constexpr double GREAT_ = 1e20;   // SolverPerformance.H:269-275
 static constexpr double SMALL_ = 1e-20;
 static constexpr double VSMALL_ = 1e-300;
@@ -44,21 +46,51 @@ __device__ __forceinline__ void hist_put(SolverScalars *sc, double *hist, int i,
     if (hist && i < sc->histCap) hist[i] = v;
 }
 
-// end of a Krylov iteration body: (nIterations++ < maxIter && !converged) || nIterations < minIter
-__device__ __forceinline__ void end_of_body(SolverScalars *sc, double *hist, double sumMag)
-{
-    sc->finalResidual = sumMag / sc->normFactor;
-    hist_put(sc, hist, sc->nIterations + 1, sc->finalResidual);
-    bool conv = check_convergence(sc);
-    int n = sc->nIterations;
-    sc->nIterations = n + 1;
-    bool cont = (n < sc->maxIter && !conv) || (n + 1 < sc->minIter);
-    if (!cont) sc->stop = 1;
-}
+// ---- scalar steps shared by the Krylov solvers ----
+// end of an iteration body whose sum|r| is sum[K]: (nIterations++ < maxIter && !converged) || nIterations < minIter
+template <int K>
+struct EndOfBody {
+    double *hist;
+    __device__ __forceinline__ void operator()(SolverScalars *sc) const
+    {
+        sc->finalResidual = sc->sum[K] / sc->normFactor;
+        hist_put(sc, hist, sc->nIterations + 1, sc->finalResidual);
+        bool conv = check_convergence(sc);
+        int n = sc->nIterations;
+        sc->nIterations = n + 1;
+        bool cont = (n < sc->maxIter && !conv) || (n + 1 < sc->minIter);
+        if (!cont) sc->stop = 1;
+    }
+};
+// beta from wArA = sum[0]
+struct BetaStep {
+    __device__ __forceinline__ void operator()(SolverScalars *s) const
+    {
+        s->wArAold = s->wArA;
+        s->wArA = s->sum[0];
+        s->beta = s->wArA / s->wArAold;
+    }
+};
+// alpha from wApA = sum[0], unless the solve is singular (checkSingularity, PCG.C:166-175); false then
+struct AlphaStep {
+    __device__ __forceinline__ bool operator()(SolverScalars *s) const
+    {
+        s->wApA = s->sum[0];
+        if (!(fabs(s->wApA) / s->normFactor > VSMALL_)) {
+            s->singular = 1;
+            s->stop = 1;
+            return false;
+        }
+        s->alpha = s->wArA / s->wApA;
+        return true;
+    }
+};
+
+// iteration bodies of a Krylov solve: maxIter + 1 (the last one's judgement always stops), at least minIter
+inline long long max_bodies(const b200ldu_controls &c) { return std::max((long long)c.maxIter + 1, (long long)c.minIter); }
 
 #define V2(p) reinterpret_cast<double2 *>(p)
 #define CV2(p) reinterpret_cast<const double2 *>(p)
-
 
 template <int NRED, class G>
 int scalar_step(Solve &S, int nPartials, G g)

@@ -13,8 +13,6 @@
 
 #include <cstdlib>
 
-#include <algorithm>
-
 #include "solver_steps.cuh"
 
 // initial residual, normFactor and the first convergence test, common to all solvers
@@ -22,12 +20,10 @@
 int init_residual(Solve &S, const double *psi, const double *b, const double *wA, double *rA, double *tmp,
                   const double *wT, double *rT)
 {
-    b200ldu_addr *a = S.m->a;
     SolverScalars *sc = S.sc;
     double *hist = S.hist;
-    const int n2 = a->L.nPad / 2;
     int np = 0;
-    TRY(ew_launch<2>(S.ctx, n2, nullptr, S.partials, &np, [=] __device__(int i, double *red) {
+    TRY(ew_launch<2>(S.ctx, S.n2, nullptr, S.partials, &np, [=] __device__(int i, double *red) {
         double2 bb = CV2(b)[i], ww = CV2(wA)[i], pp = CV2(psi)[i];
         double2 r = make_double2(__dsub_rn(bb.x, ww.x), __dsub_rn(bb.y, ww.y));
         V2(rA)[i] = r;
@@ -43,8 +39,8 @@ int init_residual(Solve &S, const double *psi, const double *b, const double *wA
         s->average = s->sum[1] / s->nCellsGlobal; // gAverage: gpuFieldCommonFunctions.C:611-635
     }));
     TRY(mat_sumA(S.m, tmp, nullptr));
-    const int nCells = a->nCells;
-    TRY(ew_launch<1>(S.ctx, n2, nullptr, S.partials, &np, [=] __device__(int i, double *red) {
+    const int nCells = S.m->a->nCells;
+    TRY(ew_launch<1>(S.ctx, S.n2, nullptr, S.partials, &np, [=] __device__(int i, double *red) {
         double avg = sc->average;
         double2 bb = CV2(b)[i], ww = CV2(wA)[i], tt = CV2(tmp)[i];
         double t0 = __dmul_rn(avg, tt.x), t1 = __dmul_rn(avg, tt.y);
@@ -62,35 +58,28 @@ int init_residual(Solve &S, const double *psi, const double *b, const double *wA
     return B200LDU_OK;
 }
 
+
 // ---------------------------------------------------------------------------
 // PCG (PCG.C:69-208)
 // ---------------------------------------------------------------------------
 int solve_pcg(Solve &S, int pk)
 {
     b200ldu_matrix *m = S.m;
-    b200ldu_addr *a = m->a;
     SolverScalars *sc = S.sc;
-    double *hist = S.hist;
-    const int *stop = &sc->stop;
-    const int n2 = a->L.nPad / 2;
     double *psi = S.psi, *b = S.src;
     double *pA = S.vec(0), *wA = S.vec(1), *rA = S.vec(2);
     if (!pA || !wA || !rA) return B200LDU_ECUDA;
 
-    TRY(mat_amul(m, false, psi, wA, 0, nullptr, nullptr, nullptr));
+    TRY(mat_amul(m, false, psi, wA, AMUL_ONLY, nullptr, nullptr, nullptr));
     TRY(init_residual(S, psi, b, wA, rA, pA));
 
     auto body = [&](long long) -> int {
         int np = 0;
         // wA = M^-1 rA ; wArA = <wA, rA>
-        TRY(mat_precondition(m, pk, false, rA, wA, true, nullptr, S.partials, &np, stop));
-        TRY(scalar_step<1>(S, np, [=] __device__(SolverScalars *s) {
-            s->wArAold = s->wArA;
-            s->wArA = s->sum[0];
-            s->beta = s->wArA / s->wArAold;
-        }));
+        TRY(mat_precondition(m, pk, false, rA, wA, true, nullptr, S.partials, &np, S.stop));
+        TRY(scalar_step<1>(S, np, BetaStep()));
         // pA = wA (first) | wA + beta*pA
-        TRY(ew_launch<0>(S.ctx, n2, stop, nullptr, nullptr, [=] __device__(int i, double *) {
+        TRY(ew_launch<0>(S.ctx, S.n2, S.stop, nullptr, nullptr, [=] __device__(int i, double *) {
             double2 w = CV2(wA)[i];
             if (sc->nIterations == 0) {
                 V2(pA)[i] = w;
@@ -101,18 +90,10 @@ int solve_pcg(Solve &S, int pk)
             }
         }));
         // wA = A pA ; wApA = <wA, pA>
-        TRY(mat_amul(m, false, pA, wA, 1, nullptr, S.partials, stop));
-        TRY(scalar_step<1>(S, a->L.nBands, [=] __device__(SolverScalars *s) {
-            s->wApA = s->sum[0];
-            if (!(fabs(s->wApA) / s->normFactor > VSMALL_)) { // checkSingularity PCG.C:170
-                s->singular = 1;
-                s->stop = 1;
-                return;
-            }
-            s->alpha = s->wArA / s->wApA;
-        }));
+        TRY(mat_amul(m, false, pA, wA, AMUL_OUT_X, nullptr, S.partials, S.stop));
+        TRY(scalar_step<1>(S, S.nBands, AlphaStep()));
         // psi += alpha pA ; rA -= alpha wA ; sum|rA|
-        TRY(ew_launch<1>(S.ctx, n2, stop, S.partials, &np, [=] __device__(int i, double *red) {
+        TRY(ew_launch<1>(S.ctx, S.n2, S.stop, S.partials, &np, [=] __device__(int i, double *red) {
             double alpha = sc->alpha;
             double2 x = CV2(psi)[i], p = CV2(pA)[i], r = CV2(rA)[i], w = CV2(wA)[i];
             x.x = fma(alpha, p.x, x.x);
@@ -123,11 +104,9 @@ int solve_pcg(Solve &S, int pk)
             V2(rA)[i] = r;
             red[0] += fabs(r.x) + fabs(r.y);
         }));
-        TRY(scalar_step<1>(S, np, [=] __device__(SolverScalars *s) { end_of_body(s, hist, s->sum[0]); }));
-        return B200LDU_OK;
+        return scalar_step<1>(S, np, EndOfBody<0>{S.hist});
     };
-    return run_iterations(S, (long long)S.c.maxIter + 1 > S.c.minIter ? (long long)S.c.maxIter + 1 : S.c.minIter,
-                          body);
+    return run_iterations(S, max_bodies(S.c), body);
 }
 
 // ---------------------------------------------------------------------------
@@ -147,38 +126,27 @@ struct PcgStepA {
     __device__ void operator()(SolverScalars *s) const
     {
         if (s->bodies > 0) {
-            end_of_body(s, hist, s->sum[1]);
+            EndOfBody<1>{hist}(s);
             if (s->stop) return;
         }
         s->psiBodies = s->bodies; // the sweep B this step opens adds the latest alpha p to psi
-        s->wArAold = s->wArA;
-        s->wArA = s->sum[0];
-        s->beta = s->wArA / s->wArAold;
+        BetaStep()(s);
     }
 };
-// scalar step B: alpha of body k (PCG.C:166-175)
+// scalar step B: alpha of body k
 struct PcgStepB {
     __device__ void operator()(SolverScalars *s) const
     {
-        s->wApA = s->sum[0];
-        if (!(fabs(s->wApA) / s->normFactor > VSMALL_)) { // checkSingularity PCG.C:170
-            s->singular = 1;
-            s->stop = 1;
-            return;
-        }
-        s->alpha = s->wArA / s->wApA;
-        s->bodies++;
+        if (AlphaStep()(s)) s->bodies++;
     }
 };
 
 int solve_pcg_fused(Solve &S, int pk)
 {
     b200ldu_matrix *m = S.m;
-    b200ldu_addr *a = m->a;
     SolverScalars *sc = S.sc;
-    double *hist = S.hist;
-    const int *stop = &sc->stop;
-    const int n2 = a->L.nPad / 2;
+    const int *stop = S.stop;
+    const int nBands = S.nBands;
     double *psi = S.psi, *b = S.src;
     double *pb[2] = {S.vec(0), S.vec(4)}, *w = S.vec(1), *rb[2] = {S.vec(2), S.vec(3)}, *z = S.vec(5);
     if (!pb[0] || !pb[1] || !w || !rb[0] || !rb[1] || !z) return B200LDU_ECUDA;
@@ -186,12 +154,12 @@ int solve_pcg_fused(Solve &S, int pk)
     const P2PRed pr = (S.ctx->nRanks > 1 && S.ctx->p2p) ? comm_p2p_red(S.ctx) : P2PRed();
     // the two sweeps leave their partials in separate buffers: a deferred step reads one while the sweep that
     // runs it writes the other
-    double *partA = S.partials, *partB = S.partials + 2 * (size_t)(a->L.nBands > S.ctx->smCount * 8 ? a->L.nBands : S.ctx->smCount * 8);
+    double *partA = S.partials, *partB = S.partials + 2 * (size_t)(nBands > S.ctx->smCount * 8 ? nBands : S.ctx->smCount * 8);
 
-    TRY(mat_amul(m, false, psi, w, 0, nullptr, nullptr, nullptr));
+    TRY(mat_amul(m, false, psi, w, AMUL_ONLY, nullptr, nullptr, nullptr));
     TRY(init_residual(S, psi, b, w, rb[0], pb[0]));
 
-    const PcgStepA gA{hist};
+    const PcgStepA gA{S.hist};
     const PcgStepB gB{};
     typedef DeferredStep<1, PcgStepB> PreA; // sweep A starts by closing sweep B of the previous body
     typedef DeferredStep<2, PcgStepA> PreB; // sweep B starts by closing sweep A of this body
@@ -202,7 +170,7 @@ int solve_pcg_fused(Solve &S, int pk)
     auto sweepAew = [&](long long k, const PreA &preA, int *npA) -> int {
         const double *rOld = rb[k & 1];
         double *rNew = rb[(k + 1) & 1];
-        return ew_launch<2>(S.ctx, n2, stop, partA, npA, [=] __device__(int i, double *red) {
+        return ew_launch<2>(S.ctx, S.n2, stop, partA, npA, [=] __device__(int i, double *red) {
             double2 r = CV2(rOld)[i];
             if (sc->bodies > 0) {
                 const double alpha = sc->alpha;
@@ -222,13 +190,13 @@ int solve_pcg_fused(Solve &S, int pk)
         }, preA);
     };
     auto preAFor = [&](long long k) {
-        return PreA{partB, a->L.nBands, sc, gB, pr, (unsigned)(2 * (k % every)), mod, k > 0 ? 1 : 0};
+        return PreA{partB, nBands, sc, gB, pr, (unsigned)(2 * (k % every)), mod, k > 0 ? 1 : 0};
     };
 
     auto body = [&](long long k) -> int {
         const double *rOld = rb[k & 1], *pPrev = pb[k & 1];
         double *rNew = rb[(k + 1) & 1], *pNew = pb[(k + 1) & 1];
-        int npA = a->L.nBands;
+        int npA = nBands;
         const PreA preA = preAFor(k);
         if (pk == 2) {
             PcgAinvOp<PreA> op;
@@ -244,7 +212,7 @@ int solve_pcg_fused(Solve &S, int pk)
         int wait = 0;
         TRY(mat_halo(m, pNew, stop, &wait)); // peer-memory path: nothing is launched, the send is fused
         const PreB preB{partA, npA, sc, gA, pr, (unsigned)(2 * (k % every) + 1), mod, 1};
-        PcgAmulOp<PreB> op{}; // zeroes the x and aux it inherits from AmulOp<1> and does not read
+        PcgAmulOp<PreB> op{}; // zeroes the x and aux it inherits from AmulOp and does not read
         op.stop = stop;
         op.partials = partB;
         op.waitHalo = wait;
@@ -254,29 +222,29 @@ int solve_pcg_fused(Solve &S, int pk)
         TRY(engine_launch_m(m, false, op));
         return B200LDU_OK;
     };
-    const long long mb = (long long)S.c.maxIter + 1 > S.c.minIter ? (long long)S.c.maxIter + 1 : S.c.minIter;
+    const long long mb = max_bodies(S.c);
     TRY(run_iterations(S, mb, body));
     // Close, enqueued after the loop and never captured: the judgement of body mb-1 always stops the solve, so of the
     // sweep A that would follow only the deferred step B (alpha of body mb-1), r = rOld - alpha w and sum|r| are
-    // needed; then the final end_of_body.  All three are no-ops once the solve has stopped.  (mb is 0 only for a
+    // needed; then the final EndOfBody.  All three are no-ops once the solve has stopped.  (mb is 0 only for a
     // negative maxIter: no body ran, nothing to close.)
     if (mb > 0) {
-        int npA = a->L.nBands;
+        int npA = nBands;
         if (pk == 2) {
-            pcg_close_kernel<PreA><<<a->L.nBands, ENGINE_THREADS, 0, S.ctx->stream>>>(a->L, rb[mb & 1], w, sc, partA,
-                                                                                       preAFor(mb));
+            pcg_close_kernel<PreA><<<nBands, ENGINE_THREADS, 0, S.ctx->stream>>>(m->a->L, rb[mb & 1], w, sc, partA,
+                                                                                 preAFor(mb));
             S.ctx->launches++;
             KERNEL_CHECK();
         } else {
             TRY(sweepAew(mb, preAFor(mb), &npA));
         }
-        TRY(scalar_step_on<2>(S, partA, npA, [=] __device__(SolverScalars *s) { end_of_body(s, hist, s->sum[1]); }));
+        TRY(scalar_step_on<2>(S, partA, npA, EndOfBody<1>{S.hist}));
     }
     // The last alpha p that no sweep B added to psi (the solve stopped at a judgement, converged or not): exactly
     // one update, also after a stop, so the stop flag does not gate it.  p of body j lives in pb[(j + 1) & 1], and the
     // last alpha is body bodies-1's.
     const double *p0 = pb[0], *p1 = pb[1];
-    return ew_launch<0>(S.ctx, n2, nullptr, nullptr, nullptr, [=] __device__(int i, double *) {
+    return ew_launch<0>(S.ctx, S.n2, nullptr, nullptr, nullptr, [=] __device__(int i, double *) {
         const int j = sc->bodies;
         if (sc->psiBodies == j) return;
         const double alpha = sc->alpha;
@@ -291,30 +259,22 @@ int solve_pcg_fused(Solve &S, int pk)
 int solve_pbicg(Solve &S, int pk)
 {
     b200ldu_matrix *m = S.m;
-    b200ldu_addr *a = m->a;
     SolverScalars *sc = S.sc;
-    double *hist = S.hist;
-    const int *stop = &sc->stop;
-    const int n2 = a->L.nPad / 2;
     double *psi = S.psi, *b = S.src;
     double *pA = S.vec(0), *wA = S.vec(1), *rA = S.vec(2), *pT = S.vec(3), *wT = S.vec(4), *rT = S.vec(5);
     if (!pA || !wA || !rA || !pT || !wT || !rT) return B200LDU_ECUDA;
-    CUDA_TRY(cudaMemsetAsync(pT, 0, sizeof(double) * (size_t)a->vecLen, S.ctx->stream)); // pT = 0 :86
+    CUDA_TRY(cudaMemsetAsync(pT, 0, sizeof(double) * (size_t)m->a->vecLen, S.ctx->stream)); // pT = 0 :86
 
-    TRY(mat_amul(m, false, psi, wA, 0, nullptr, nullptr, nullptr));
-    TRY(mat_amul(m, true, psi, wT, 0, nullptr, nullptr, nullptr));
+    TRY(mat_amul(m, false, psi, wA, AMUL_ONLY, nullptr, nullptr, nullptr));
+    TRY(mat_amul(m, true, psi, wT, AMUL_ONLY, nullptr, nullptr, nullptr));
     TRY(init_residual(S, psi, b, wA, rA, pA, wT, rT));
 
     auto body = [&](long long) -> int {
         int np = 0;
-        TRY(mat_precondition(m, pk, true, rT, wT, false, nullptr, nullptr, nullptr, stop));
-        TRY(mat_precondition(m, pk, false, rA, wA, true, rT, S.partials, &np, stop)); // wArT = <wA, rT>
-        TRY(scalar_step<1>(S, np, [=] __device__(SolverScalars *s) {
-            s->wArAold = s->wArA;
-            s->wArA = s->sum[0];
-            s->beta = s->wArA / s->wArAold;
-        }));
-        TRY(ew_launch<0>(S.ctx, n2, stop, nullptr, nullptr, [=] __device__(int i, double *) {
+        TRY(mat_precondition(m, pk, true, rT, wT, false, nullptr, nullptr, nullptr, S.stop));
+        TRY(mat_precondition(m, pk, false, rA, wA, true, rT, S.partials, &np, S.stop)); // wArT = <wA, rT>
+        TRY(scalar_step<1>(S, np, BetaStep()));
+        TRY(ew_launch<0>(S.ctx, S.n2, S.stop, nullptr, nullptr, [=] __device__(int i, double *) {
             double2 w = CV2(wA)[i], wt = CV2(wT)[i];
             if (sc->nIterations == 0) {
                 V2(pA)[i] = w;
@@ -326,18 +286,10 @@ int solve_pbicg(Solve &S, int pk)
                 V2(pT)[i] = make_double2(fma(beta, pt.x, wt.x), fma(beta, pt.y, wt.y));
             }
         }));
-        TRY(mat_amul(m, true, pT, wT, 0, nullptr, nullptr, stop));
-        TRY(mat_amul(m, false, pA, wA, 3, pT, S.partials, stop)); // wApT = <wA, pT>
-        TRY(scalar_step<1>(S, a->L.nBands, [=] __device__(SolverScalars *s) {
-            s->wApA = s->sum[0];
-            if (!(fabs(s->wApA) / s->normFactor > VSMALL_)) {
-                s->singular = 1;
-                s->stop = 1;
-                return;
-            }
-            s->alpha = s->wArA / s->wApA;
-        }));
-        TRY(ew_launch<1>(S.ctx, n2, stop, S.partials, &np, [=] __device__(int i, double *red) {
+        TRY(mat_amul(m, true, pT, wT, AMUL_ONLY, nullptr, nullptr, S.stop));
+        TRY(mat_amul(m, false, pA, wA, AMUL_OUT_AUX, pT, S.partials, S.stop)); // wApT = <wA, pT>
+        TRY(scalar_step<1>(S, S.nBands, AlphaStep()));
+        TRY(ew_launch<1>(S.ctx, S.n2, S.stop, S.partials, &np, [=] __device__(int i, double *red) {
             double alpha = sc->alpha;
             double2 x = CV2(psi)[i], p = CV2(pA)[i], r = CV2(rA)[i], w = CV2(wA)[i];
             double2 rt = CV2(rT)[i], wt = CV2(wT)[i];
@@ -352,11 +304,9 @@ int solve_pbicg(Solve &S, int pk)
             V2(rT)[i] = rt;
             red[0] += fabs(r.x) + fabs(r.y);
         }));
-        TRY(scalar_step<1>(S, np, [=] __device__(SolverScalars *s) { end_of_body(s, hist, s->sum[0]); }));
-        return B200LDU_OK;
+        return scalar_step<1>(S, np, EndOfBody<0>{S.hist});
     };
-    return run_iterations(S, (long long)S.c.maxIter + 1 > S.c.minIter ? (long long)S.c.maxIter + 1 : S.c.minIter,
-                          body);
+    return run_iterations(S, max_bodies(S.c), body);
 }
 
 // ---------------------------------------------------------------------------
@@ -365,26 +315,23 @@ int solve_pbicg(Solve &S, int pk)
 int solve_pbicgstab(Solve &S, int pk)
 {
     b200ldu_matrix *m = S.m;
-    b200ldu_addr *a = m->a;
     SolverScalars *sc = S.sc;
     double *hist = S.hist;
-    const int *stop = &sc->stop;
-    const int n2 = a->L.nPad / 2;
     const int quirk = S.c.bicgstabRefQuirk;
     double *psi = S.psi, *b = S.src;
     double *pA = S.vec(0), *yA = S.vec(1), *rA = S.vec(2), *AyA = S.vec(3), *sA = S.vec(4), *zA = S.vec(5),
            *tA = S.vec(6), *rA0 = S.vec(7);
     if (!pA || !yA || !rA || !AyA || !sA || !zA || !tA || !rA0) return B200LDU_ECUDA;
 
-    TRY(mat_amul(m, false, psi, yA, 0, nullptr, nullptr, nullptr));
+    TRY(mat_amul(m, false, psi, yA, AMUL_ONLY, nullptr, nullptr, nullptr));
     TRY(init_residual(S, psi, b, yA, rA, pA));
-    CUDA_TRY(cudaMemcpyAsync(rA0, rA, sizeof(double) * (size_t)a->vecLen, cudaMemcpyDeviceToDevice,
+    CUDA_TRY(cudaMemcpyAsync(rA0, rA, sizeof(double) * (size_t)m->a->vecLen, cudaMemcpyDeviceToDevice,
                              S.ctx->stream)); // rA0 = rA :127
 
     auto body = [&](long long) -> int {
         int np = 0;
         // rA0rA = <rA0, rA>
-        TRY(ew_launch<1>(S.ctx, n2, stop, S.partials, &np, [=] __device__(int i, double *red) {
+        TRY(ew_launch<1>(S.ctx, S.n2, S.stop, S.partials, &np, [=] __device__(int i, double *red) {
             double2 x = CV2(rA0)[i], y = CV2(rA)[i];
             red[0] += x.x * y.x + x.y * y.y;
         }));
@@ -406,7 +353,7 @@ int solve_pbicgstab(Solve &S, int pk)
             }
         }));
         // pA = rA (first) | rA + beta*(pA - omega*AyA)
-        TRY(ew_launch<0>(S.ctx, n2, stop, nullptr, nullptr, [=] __device__(int i, double *) {
+        TRY(ew_launch<0>(S.ctx, S.n2, S.stop, nullptr, nullptr, [=] __device__(int i, double *) {
             double2 r = CV2(rA)[i];
             if (sc->nIterations == 0) {
                 V2(pA)[i] = r;
@@ -417,11 +364,11 @@ int solve_pbicgstab(Solve &S, int pk)
                 V2(pA)[i] = make_double2(fma(beta, r1x, r.x), fma(beta, r1y, r.y));
             }
         }));
-        TRY(mat_precondition(m, pk, false, pA, yA, false, nullptr, nullptr, nullptr, stop));
-        TRY(mat_amul(m, false, yA, AyA, 3, rA0, S.partials, stop)); // rA0AyA
-        TRY(scalar_step<1>(S, a->L.nBands, [=] __device__(SolverScalars *s) { s->alpha = s->rA0rA / s->sum[0]; }));
+        TRY(mat_precondition(m, pk, false, pA, yA, false, nullptr, nullptr, nullptr, S.stop));
+        TRY(mat_amul(m, false, yA, AyA, AMUL_OUT_AUX, rA0, S.partials, S.stop)); // rA0AyA
+        TRY(scalar_step<1>(S, S.nBands, [=] __device__(SolverScalars *s) { s->alpha = s->rA0rA / s->sum[0]; }));
         // sA = rA - alpha*AyA ; psi += alpha*yA (both exits of the body need it) ; sum|sA|
-        TRY(ew_launch<1>(S.ctx, n2, stop, S.partials, &np, [=] __device__(int i, double *red) {
+        TRY(ew_launch<1>(S.ctx, S.n2, S.stop, S.partials, &np, [=] __device__(int i, double *red) {
             double alpha = sc->alpha;
             double2 r = CV2(rA)[i], ay = CV2(AyA)[i], x = CV2(psi)[i], y = CV2(yA)[i];
             double2 s2 = make_double2(fma(-alpha, ay.x, r.x), fma(-alpha, ay.y, r.y));
@@ -437,10 +384,10 @@ int solve_pbicgstab(Solve &S, int pk)
                 s->stop = 1;
             }
         }));
-        TRY(mat_precondition(m, pk, false, sA, zA, false, nullptr, nullptr, nullptr, stop));
-        TRY(mat_amul(m, false, zA, tA, 4, sA, S.partials, stop)); // tAtA, tAsA
-        TRY(scalar_step<2>(S, a->L.nBands, [=] __device__(SolverScalars *s) { s->omega = s->sum[1] / s->sum[0]; }));
-        TRY(ew_launch<1>(S.ctx, n2, stop, S.partials, &np, [=] __device__(int i, double *red) {
+        TRY(mat_precondition(m, pk, false, sA, zA, false, nullptr, nullptr, nullptr, S.stop));
+        TRY(mat_amul(m, false, zA, tA, AMUL_OUT_OUT_OUT_AUX, sA, S.partials, S.stop)); // tAtA, tAsA
+        TRY(scalar_step<2>(S, S.nBands, [=] __device__(SolverScalars *s) { s->omega = s->sum[1] / s->sum[0]; }));
+        TRY(ew_launch<1>(S.ctx, S.n2, S.stop, S.partials, &np, [=] __device__(int i, double *red) {
             double omega = sc->omega;
             const double *second = quirk ? yA : zA; // PBiCGStab.C:263-270 passes yA
             double2 x = CV2(psi)[i], z = CV2(second)[i], s2 = CV2(sA)[i], t = CV2(tA)[i];
@@ -449,11 +396,9 @@ int solve_pbicgstab(Solve &S, int pk)
             V2(rA)[i] = r;
             red[0] += fabs(r.x) + fabs(r.y);
         }));
-        TRY(scalar_step<1>(S, np, [=] __device__(SolverScalars *s) { end_of_body(s, hist, s->sum[0]); }));
-        return B200LDU_OK;
+        return scalar_step<1>(S, np, EndOfBody<0>{hist});
     };
-    return run_iterations(S, (long long)S.c.maxIter + 1 > S.c.minIter ? (long long)S.c.maxIter + 1 : S.c.minIter,
-                          body);
+    return run_iterations(S, max_bodies(S.c), body);
 }
 
 // ---------------------------------------------------------------------------
@@ -462,33 +407,30 @@ int solve_pbicgstab(Solve &S, int pk)
 int solve_smooth(Solve &S)
 {
     b200ldu_matrix *m = S.m;
-    b200ldu_addr *a = m->a;
-    SolverScalars *sc = S.sc;
     double *hist = S.hist;
-    const int *stop = &sc->stop;
     double *b = S.src;
     double *buf[2] = {S.psi, S.vec(0)};
     double *tmp = S.vec(1), *Apsi = S.vec(2);
     if (!buf[1] || !tmp || !Apsi) return B200LDU_ECUDA;
     const double omega = S.c.omega;
+    const int nSweeps = S.c.nSweeps;
+    // psi ping-pongs between buf[0] and buf[1], one sweep at a time; nIterations counts sweeps
+    S.result = SolveResult{{buf[0], buf[1]}, 1, nSweeps > 0 ? nSweeps : 1};
     long long sweepsDone = 0;
 
-    if (S.c.nSweeps < 0) { // fixed number of sweeps, no residual evaluation (:88-110)
-        int ns = -S.c.nSweeps;
-        for (int s = 0; s < ns; s++, sweepsDone++)
+    if (nSweeps < 0) { // fixed number of sweeps, no residual evaluation (:88-110); solve_banded seeded nIterations
+        S.result.histEvery = 0;
+        for (int s = 0; s < -nSweeps; s++, sweepsDone++)
             TRY(mat_jacobi(m, omega, buf[sweepsDone & 1], b, buf[(sweepsDone + 1) & 1], nullptr));
-        S.resultBuf = buf[sweepsDone & 1];
-        S.fixedSweeps = ns;
         return B200LDU_OK;
     }
-    TRY(mat_amul(m, false, S.psi, Apsi, 0, nullptr, nullptr, nullptr));
+    TRY(mat_amul(m, false, S.psi, Apsi, AMUL_ONLY, nullptr, nullptr, nullptr));
     TRY(init_residual(S, S.psi, b, Apsi, tmp, buf[1]));
-    const int nSweeps = S.c.nSweeps;
     auto body = [&](long long) -> int {
         for (int s = 0; s < nSweeps; s++, sweepsDone++)
-            TRY(mat_jacobi(m, omega, buf[sweepsDone & 1], b, buf[(sweepsDone + 1) & 1], stop));
-        TRY(mat_residual(m, buf[sweepsDone & 1], b, tmp, true, S.partials, stop));
-        TRY(scalar_step<1>(S, a->L.nBands, [=] __device__(SolverScalars *s) {
+            TRY(mat_jacobi(m, omega, buf[sweepsDone & 1], b, buf[(sweepsDone + 1) & 1], S.stop));
+        TRY(mat_residual(m, buf[sweepsDone & 1], b, tmp, true, S.partials, S.stop));
+        return scalar_step<1>(S, S.nBands, [=] __device__(SolverScalars *s) {
             s->finalResidual = s->sum[0] / s->normFactor;
             int k = s->nIterations / (nSweeps > 0 ? nSweeps : 1) + 1;
             hist_put(s, hist, k, s->finalResidual);
@@ -496,235 +438,235 @@ int solve_smooth(Solve &S)
             s->nIterations += nSweeps; // ((nIterations += nSweeps) < maxIter && !conv) || nIterations < minIter
             bool cont = (s->nIterations < s->maxIter && !conv) || s->nIterations < s->minIter;
             if (!cont) s->stop = 1;
-        }));
-        return B200LDU_OK;
+        });
     };
     int per = nSweeps > 0 ? nSweeps : 1;
     long long maxBodies = ((long long)(S.c.maxIter > S.c.minIter ? S.c.maxIter : S.c.minIter) + per - 1) / per + 1;
-    TRY(run_iterations(S, maxBodies, body));
-    S.sweepsPerIteration = 1; // nIterations counts sweeps; the buffer is picked after the read-back
-    S.smoothBuf[0] = buf[0];
-    S.smoothBuf[1] = buf[1];
-    return B200LDU_OK;
+    return run_iterations(S, maxBodies, body);
 }
 
-// diagonalSolver.C:62-81
+// diagonalSolver.C:62-81; solve_banded seeded converged = 1
 int solve_diagonal(Solve &S)
 {
     const double *d = S.m->d_diag;
     double *psi = S.psi;
     const double *b = S.src;
-    return ew_launch<0>(S.ctx, S.m->a->L.nPad / 2, nullptr, nullptr, nullptr, [=] __device__(int i, double *) {
+    S.result.histEvery = 0;
+    return ew_launch<0>(S.ctx, S.n2, nullptr, nullptr, nullptr, [=] __device__(int i, double *) {
         double2 bb = CV2(b)[i], dd = CV2(d)[i];
         V2(psi)[i] = make_double2(__ddiv_rn(bb.x, dd.x), __ddiv_rn(bb.y, dd.y));
     });
 }
 
-double *Solve::vec(int k)
+int gamg_solve(Solve &S, b200ldu_gamg *g); // gamg.cu
+
+// ---------------------------------------------------------------------------
+// the solve session
+// ---------------------------------------------------------------------------
+static thread_local int solveDepth = 0; // a solve nested in another one (GAMG coarsest level) polls its own flags
+
+Solve::Solve(b200ldu_matrix *mat, const b200ldu_controls &controls, double *psi_b, double *src_b, int histCapacity,
+             int nIterations0, int converged0)
+    : m(mat), ctx(mat->a->ctx), sc((SolverScalars *)mat->d_scal), stop(&sc->stop), n2(mat->a->L.nPad / 2),
+      nBands(mat->a->L.nBands), partials(mat->d_partials), psi(psi_b), src(src_b), c(controls), histCap(histCapacity)
 {
-    return k < MAT_NWORK ? banded_vec(m->a, m->mem, MAT_WORK + k) : nullptr;
+    result.buf[0] = result.buf[1] = psi;
+    rc = open(nIterations0, converged0);
 }
 
-int gamg_solve(Solve &S, b200ldu_gamg *g, const char *smoother); // gamg.cu
-
-// run-time selection: lduMatrixSolver.C:43-140.  psi_b / src_b are banded vectors.
-int solve_banded(b200ldu_matrix *m, const char *solver, const char *pre, const b200ldu_controls *controls,
-                 b200ldu_gamg *gamg, double *psi_b, double *src_b, b200ldu_perf *perf, double *hist_h,
-                 int histCap, double **resultBuf)
+int Solve::open(int nIterations0, int converged0)
 {
-    b200ldu_addr *a = m->a;
-    b200ldu_ctx *ctx = a->ctx;
-    Solve S;
-    S.m = m;
-    S.ctx = ctx;
-    S.sc = (SolverScalars *)m->d_scal;
-    S.partials = m->d_partials;
-    S.psi = psi_b;
-    S.src = src_b;
-    if (controls)
-        S.c = *controls;
-    else
-        b200ldu_controls_default(&S.c);
-    memset(perf, 0, sizeof(*perf));
-    *resultBuf = psi_b;
-
-    // residual history buffer on the device
-    if (histCap > 0 && hist_h) TRY(m->mem.slot(MAT_HIST, S.hist, (size_t)histCap));
-    // pinned flags + events
-    void *pin = nullptr;
-    TRY(ctx_pinned(ctx, 4096, &pin));
-    // a solve nested in another one (GAMG coarsest level) polls its own pair of flags
-    static thread_local int depth = 0;
-    struct Depth {
-        int &d;
-        Depth(int &x) : d(x) { d++; }
-        ~Depth() { d--; }
-    } depthGuard(depth);
-    if (depth > 8) {
+    if (histCap > 0) TRY(m->mem.slot(MAT_HIST, hist, (size_t)histCap));
+    entered_ = true;
+    if (++solveDepth > SOLVE_MAX_DEPTH) {
         b200_set_error("solve: nesting too deep");
         return B200LDU_EINVAL;
     }
-    S.pinnedFlags = (int *)pin + 2 * (depth - 1);
-    S.pinnedFlags[0] = S.pinnedFlags[1] = 0;
-    CUDA_TRY(cudaEventCreateWithFlags(&S.ev[0], cudaEventDisableTiming));
-    CUDA_TRY(cudaEventCreateWithFlags(&S.ev[1], cudaEventDisableTiming));
+    pinnedFlags = ctx->pinned->flags[solveDepth - 1];
+    pinnedFlags[0] = pinnedFlags[1] = 0;
+    CUDA_TRY(cudaEventCreateWithFlags(&ev[0], cudaEventDisableTiming));
+    CUDA_TRY(cudaEventCreateWithFlags(&ev[1], cudaEventDisableTiming));
 
     // CUDA graphs need a capturable stream: if the context runs on the legacy default stream the
     // solve moves to the context's own stream, ordered against the caller's stream by events
-    {
-        const char *ev = getenv("B200LDU_GRAPH");
-        S.useGraph = !(ev && atoi(ev) == 0) && (ctx->nRanks == 1 || ctx->p2p);
-    }
-    cudaStream_t userStream = ctx->stream;
-    const bool swapStream = S.useGraph && ctx->ownStream && userStream != ctx->ownStream;
-    if (swapStream) {
-        CUDA_TRY(cudaEventRecord(S.ev[0], userStream));
-        CUDA_TRY(cudaStreamWaitEvent(ctx->ownStream, S.ev[0], 0));
+    const char *env = getenv("B200LDU_GRAPH");
+    useGraph = !(env && atoi(env) == 0) && (ctx->nRanks == 1 || ctx->p2p);
+    if (useGraph && ctx->ownStream && ctx->stream != ctx->ownStream) {
+        CUDA_TRY(cudaEventRecord(ev[0], ctx->stream));
+        CUDA_TRY(cudaStreamWaitEvent(ctx->ownStream, ev[0], 0));
+        userStream_ = ctx->stream;
+        swapped_ = true;
         ctx->stream = ctx->ownStream;
     }
-    struct StreamRestore {
-        b200ldu_ctx *c;
-        cudaStream_t user;
-        bool on;
-        ~StreamRestore()
-        {
-            if (!on) return;
-            cudaEvent_t e;
-            if (cudaEventCreateWithFlags(&e, cudaEventDisableTiming) == cudaSuccess) {
-                cudaEventRecord(e, c->ownStream);
-                cudaStreamWaitEvent(user, e, 0);
-                cudaEventDestroy(e);
-            }
-            c->stream = user;
-        }
-    } restore{ctx, userStream, swapStream};
 
+    const b200ldu_addr *a = m->a;
     SolverScalars h;
     memset(&h, 0, sizeof(h));
     h.wArA = GREAT_; // PCG.C:88
     h.wArAold = GREAT_;
-    h.tolerance = S.c.tolerance;
-    h.relTol = S.c.relTol;
-    h.maxIter = S.c.maxIter;
-    h.minIter = S.c.minIter;
-    h.histCap = S.hist ? histCap : 0;
-    h.nSweeps = S.c.nSweeps;
+    h.tolerance = c.tolerance;
+    h.relTol = c.relTol;
+    h.maxIter = c.maxIter;
+    h.minIter = c.minIter;
+    h.histCap = histCap;
+    h.nSweeps = c.nSweeps;
     h.nCellsGlobal = a->nCellsGlobal > 0 ? a->nCellsGlobal : (double)a->nCells; // all-reduced at addr_create
-    CUDA_TRY(cudaMemcpyAsync(S.sc, &h, sizeof(h), cudaMemcpyHostToDevice, ctx->stream));
+    h.nIterations = nIterations0;
+    h.converged = converged0;
+    CUDA_TRY(cudaMemcpyAsync(sc, &h, sizeof(h), cudaMemcpyHostToDevice, ctx->stream));
+    return B200LDU_OK;
+}
 
-    int rc = B200LDU_OK;
-    bool diagonalOnly = (a->nFaces == 0 && a->L.nRecv == 0);
+Solve::~Solve()
+{
+    if (swapped_) {
+        if (cudaEventRecord(ev[0], ctx->ownStream) == cudaSuccess) cudaStreamWaitEvent(userStream_, ev[0], 0);
+        ctx->stream = userStream_;
+    }
+    if (ev[0]) cudaEventDestroy(ev[0]);
+    if (ev[1]) cudaEventDestroy(ev[1]);
+    if (entered_) solveDepth--;
+}
+
+int Solve::finish(b200ldu_perf *perf, double *hist_h, double **psiOut)
+{
+    // read back the scalars (one synchronisation per solve)
+    PinnedArea *pin = ctx->pinned;
+    CUDA_TRY(cudaMemcpyAsync(&pin->scalars, sc, sizeof(SolverScalars), cudaMemcpyDeviceToHost, ctx->stream));
+    pin->peerErr = 0;
+    if (ctx->d_seq) // a bounded wait on a peer's flag gave up (engine.cuh spin_until)
+        CUDA_TRY(cudaMemcpyAsync(&pin->peerErr, ctx->d_seq + 7, sizeof(pin->peerErr), cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    int status = B200LDU_OK;
+    if (pin->peerErr) {
+        b200_set_error("solve: timed out waiting for a peer GPU's halo / all-reduce flag (a rank died or did not "
+                       "enter the matching solve)");
+        status = B200LDU_ENCCL;
+    }
+    const SolverScalars &h = pin->scalars;
+    perf->initialResidual = h.initialResidual;
+    perf->finalResidual = h.finalResidual;
+    perf->normFactor = h.normFactor;
+    perf->nIterations = h.nIterations;
+    perf->converged = h.converged;
+    perf->singular = h.singular;
+    *psiOut = result.buf[((long long)h.nIterations * result.sweepsPerIteration) & 1];
+    if (hist) {
+        int k = result.histEvery > 0 ? h.nIterations / result.histEvery + 1 : 0;
+        if (k > histCap) k = histCap;
+        if (k > 0) CUDA_TRY(cudaMemcpy(hist_h, hist, sizeof(double) * (size_t)k, cudaMemcpyDeviceToHost));
+        for (int i = k; i < histCap; i++) hist_h[i] = NAN;
+    }
+    return status;
+}
+
+// ---------------------------------------------------------------------------
+// run-time selection: lduMatrixSolver.C:43-140
+// ---------------------------------------------------------------------------
+enum SolverBody { BODY_DIAGONAL, BODY_PCG, BODY_PCG_FUSED, BODY_PBICG, BODY_PBICGSTAB, BODY_SMOOTH, BODY_GAMG };
+
+// The solver body to run, its preconditioner kind *pk and perf->solverName.  Allocates and enqueues nothing, so a
+// refused selection leaves psi and the caller's history as they were.
+static int select_solver(const b200ldu_matrix *m, const char *solver, const char *pre, const b200ldu_gamg *gamg,
+                         b200ldu_perf *perf, SolverBody *body, int *pk)
+{
+    const b200ldu_addr *a = m->a;
     const char *sv = solver ? solver : "";
-    char pname[32] = "";
-    if (diagonalOnly || !strcmp(sv, "diagonal")) {
+    if ((a->nFaces == 0 && a->L.nRecv == 0) || !strcmp(sv, "diagonal")) {
         strcpy(perf->solverName, "diagonal");
-        rc = solve_diagonal(S);
-        perf->converged = 1;
-        S.noScalars = true;
-    } else {
-        // ICCG / BICCG wrappers (ICCG.C:40-51)
-        if (!strcmp(sv, "ICCG")) {
-            sv = "PCG";
-            pre = "DIC";
-        } else if (!strcmp(sv, "BICCG")) {
-            sv = "PBiCG";
-            pre = "DILU";
-        }
-        if (!strcmp(sv, "PCG") || !strcmp(sv, "PBiCG") || !strcmp(sv, "PBiCGStab")) {
-            // solver::New looks the name up in the table of the matrix kind first (lduMatrixSolver.C:70-133); the
-            // preconditioner is selected inside solve() from the tables of the same kind: DIC symmetric, DILU
-            // asymmetric, AINV / diagonal / none both (DICPreconditioner.C:35, DILUPreconditioner.C:35, ...)
-            const bool wantSym = !strcmp(sv, "PCG");
-            int pk = -1;
-            if (wantSym != (bool)m->symmetric) {
-                b200_set_error("%s is registered for %s matrices only (PCG.C:36, PBiCG.C:36, PBiCGStab.C:36)", sv,
-                               wantSym ? "symmetric" : "asymmetric");
-                rc = B200LDU_EMATRIX;
-            } else if ((pk = precond_kind(pre, pname)) < 0) {
-                rc = B200LDU_ENOPRECOND;
-            } else if (pre && ((!strcmp(pre, "DILU") && m->symmetric) || (!strcmp(pre, "DIC") && !m->symmetric))) {
-                b200_set_error("Unknown %s matrix preconditioner %s; valid %s matrix preconditioners: (AINV %s diagonal none)",
-                               m->symmetric ? "symmetric" : "asymmetric", pre, m->symmetric ? "symmetric" : "asymmetric",
-                               m->symmetric ? "DIC" : "DILU");
-                rc = B200LDU_ENOPRECOND;
-            } else {
-                snprintf(perf->solverName, sizeof(perf->solverName), "%s%s", pname, sv);
-                if (!strcmp(sv, "PCG")) {
-                    // the fused form needs every exchange inside the kernels: the peer-memory halo (or no halo)
-                    // and the peer-memory all-reduce (or one rank); otherwise -- cyclic patches, NCCL fall-back --
-                    // and with B200LDU_PCG_FUSED=0 the reference's op list runs kernel by kernel
-                    const char *ev = getenv("B200LDU_PCG_FUSED");
-                    bool fused = !(ev && atoi(ev) == 0) && (a->L.nRecv == 0 || a->p2pHalo) && (ctx->nRanks == 1 || ctx->p2p);
-                    rc = fused ? solve_pcg_fused(S, pk) : solve_pcg(S, pk);
-                } else if (!strcmp(sv, "PBiCG")) {
-                    rc = solve_pbicg(S, pk);
-                } else {
-                    rc = solve_pbicgstab(S, pk);
-                }
-            }
-        } else if (!strcmp(sv, "smoothSolver")) {
-            if (!smoother_ok(pre))
-                rc = B200LDU_ENOPRECOND;
-            else {
-                strcpy(perf->solverName, "smoothSolver");
-                rc = solve_smooth(S);
-            }
-        } else if (!strcmp(sv, "GAMG")) {
-            if (!smoother_ok(pre))
-                rc = B200LDU_ENOPRECOND;
-            else if (!gamg) {
-                b200_set_error("GAMG needs an agglomeration handle (b200ldu_gamg_create)");
-                rc = B200LDU_EINVAL;
-            } else {
-                strcpy(perf->solverName, "GAMG");
-                rc = gamg_solve(S, gamg, pre);
-            }
-        } else {
-            b200_set_error("Unknown %s solver %s; valid solvers: (BICCG GAMG ICCG PBiCG PBiCGStab PCG "
-                           "diagonal smoothSolver)",
-                           m->symmetric ? "symmetric" : "asymmetric", sv);
-            rc = B200LDU_ENOSOLVER;
-        }
+        *body = BODY_DIAGONAL;
+        return B200LDU_OK;
     }
-    if (rc == B200LDU_OK) {
-        // read back the scalars (one synchronisation per solve)
-        SolverScalars *hp = (SolverScalars *)((char *)pin + 1024);
-        CUDA_TRY(cudaMemcpyAsync(hp, S.sc, sizeof(SolverScalars), cudaMemcpyDeviceToHost, ctx->stream));
-        unsigned long long *peerErr = (unsigned long long *)((char *)pin + 2048);
-        *peerErr = 0;
-        if (ctx->d_seq) // a bounded wait on a peer's flag gave up (engine.cuh spin_until)
-            CUDA_TRY(cudaMemcpyAsync(peerErr, ctx->d_seq + 7, sizeof(*peerErr), cudaMemcpyDeviceToHost, ctx->stream));
-        CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-        if (*peerErr) {
-            b200_set_error("solve: timed out waiting for a peer GPU's halo / all-reduce flag (a rank died or did not "
-                           "enter the matching solve)");
-            rc = B200LDU_ENCCL;
-        }
-        if (!S.noScalars) {
-            perf->initialResidual = hp->initialResidual;
-            perf->finalResidual = hp->finalResidual;
-            perf->normFactor = hp->normFactor;
-            perf->nIterations = hp->nIterations;
-            perf->converged = hp->converged;
-            perf->singular = hp->singular;
-        }
-        if (S.fixedSweeps) perf->nIterations = S.fixedSweeps;
-        if (S.sweepsPerIteration) S.resultBuf = S.smoothBuf[((long long)perf->nIterations * S.sweepsPerIteration) & 1];
-        if (S.resultBuf) *resultBuf = S.resultBuf;
-        if (S.hist && hist_h) {
-            int k = perf->nIterations + 1;
-            if (!strcmp(perf->solverName, "smoothSolver") && S.c.nSweeps > 0) k = perf->nIterations / S.c.nSweeps + 1;
-            if (k > histCap) k = histCap;
-            if (S.noScalars || S.fixedSweeps) k = 0;
-            if (k > 0) CUDA_TRY(cudaMemcpy(hist_h, S.hist, sizeof(double) * (size_t)k, cudaMemcpyDeviceToHost));
-            for (int i = k; i < histCap; i++) hist_h[i] = NAN;
-        }
-    } else {
-        cudaStreamSynchronize(ctx->stream);
+    // ICCG / BICCG wrappers (ICCG.C:40-51)
+    if (!strcmp(sv, "ICCG")) {
+        sv = "PCG";
+        pre = "DIC";
+    } else if (!strcmp(sv, "BICCG")) {
+        sv = "PBiCG";
+        pre = "DILU";
     }
-    cudaEventDestroy(S.ev[0]);
-    cudaEventDestroy(S.ev[1]);
-    return rc;
+    if (!strcmp(sv, "smoothSolver") || !strcmp(sv, "GAMG")) {
+        if (!smoother_ok(pre)) return B200LDU_ENOPRECOND;
+        *body = strcmp(sv, "GAMG") ? BODY_SMOOTH : BODY_GAMG;
+        if (*body == BODY_GAMG && !gamg) {
+            b200_set_error("GAMG needs an agglomeration handle (b200ldu_gamg_create)");
+            return B200LDU_EINVAL;
+        }
+        strcpy(perf->solverName, sv);
+        return B200LDU_OK;
+    }
+    if (strcmp(sv, "PCG") && strcmp(sv, "PBiCG") && strcmp(sv, "PBiCGStab")) {
+        b200_set_error("Unknown %s solver %s; valid solvers: (BICCG GAMG ICCG PBiCG PBiCGStab PCG "
+                       "diagonal smoothSolver)",
+                       m->symmetric ? "symmetric" : "asymmetric", sv);
+        return B200LDU_ENOSOLVER;
+    }
+    // solver::New looks the name up in the table of the matrix kind first (lduMatrixSolver.C:70-133); the
+    // preconditioner is selected inside solve() from the tables of the same kind: DIC symmetric, DILU
+    // asymmetric, AINV / diagonal / none both (DICPreconditioner.C:35, DILUPreconditioner.C:35, ...)
+    const bool wantSym = !strcmp(sv, "PCG");
+    char pname[32] = "";
+    if (wantSym != (bool)m->symmetric) {
+        b200_set_error("%s is registered for %s matrices only (PCG.C:36, PBiCG.C:36, PBiCGStab.C:36)", sv,
+                       wantSym ? "symmetric" : "asymmetric");
+        return B200LDU_EMATRIX;
+    }
+    if ((*pk = precond_kind(pre, pname)) < 0) return B200LDU_ENOPRECOND;
+    if (pre && ((!strcmp(pre, "DILU") && m->symmetric) || (!strcmp(pre, "DIC") && !m->symmetric))) {
+        b200_set_error("Unknown %s matrix preconditioner %s; valid %s matrix preconditioners: (AINV %s diagonal none)",
+                       m->symmetric ? "symmetric" : "asymmetric", pre, m->symmetric ? "symmetric" : "asymmetric",
+                       m->symmetric ? "DIC" : "DILU");
+        return B200LDU_ENOPRECOND;
+    }
+    snprintf(perf->solverName, sizeof(perf->solverName), "%s%s", pname, sv);
+    if (wantSym) {
+        // the fused form needs every exchange inside the kernels: the peer-memory halo (or no halo)
+        // and the peer-memory all-reduce (or one rank); otherwise -- cyclic patches, NCCL fall-back --
+        // and with B200LDU_PCG_FUSED=0 the reference's op list runs kernel by kernel
+        const char *ev = getenv("B200LDU_PCG_FUSED");
+        const bool fused = !(ev && atoi(ev) == 0) && (a->L.nRecv == 0 || a->p2pHalo) &&
+                           (a->ctx->nRanks == 1 || a->ctx->p2p);
+        *body = fused ? BODY_PCG_FUSED : BODY_PCG;
+    } else {
+        *body = strcmp(sv, "PBiCG") ? BODY_PBICGSTAB : BODY_PBICG;
+    }
+    return B200LDU_OK;
+}
+
+// psi_b / src_b are banded vectors; *resultBuf receives the banded vector that holds the solution
+int solve_banded(b200ldu_matrix *m, const char *solver, const char *pre, const b200ldu_controls *controls,
+                 b200ldu_gamg *gamg, double *psi_b, double *src_b, b200ldu_perf *perf, double *hist_h,
+                 int histCap, double **resultBuf)
+{
+    memset(perf, 0, sizeof(*perf));
+    *resultBuf = psi_b;
+    SolverBody body;
+    int pk = 0;
+    TRY(select_solver(m, solver, pre, gamg, perf, &body, &pk));
+    b200ldu_controls c;
+    if (controls)
+        c = *controls;
+    else
+        b200ldu_controls_default(&c);
+    // what the solvers that run no scalar step report: the diagonal solver converged, fixed sweeps count themselves
+    const int nIterations0 = body == BODY_SMOOTH && c.nSweeps < 0 ? -c.nSweeps : 0;
+    Solve S(m, c, psi_b, src_b, hist_h ? histCap : 0, nIterations0, body == BODY_DIAGONAL);
+    TRY(S.rc);
+    int rc = B200LDU_ECUDA;
+    switch (body) {
+    case BODY_DIAGONAL: rc = solve_diagonal(S); break;
+    case BODY_PCG: rc = solve_pcg(S, pk); break;
+    case BODY_PCG_FUSED: rc = solve_pcg_fused(S, pk); break;
+    case BODY_PBICG: rc = solve_pbicg(S, pk); break;
+    case BODY_PBICGSTAB: rc = solve_pbicgstab(S, pk); break;
+    case BODY_SMOOTH: rc = solve_smooth(S); break;
+    case BODY_GAMG: rc = gamg_solve(S, gamg); break;
+    }
+    if (rc != B200LDU_OK) {
+        cudaStreamSynchronize(S.ctx->stream);
+        return rc;
+    }
+    return S.finish(perf, hist_h, resultBuf);
 }
 
 extern "C" int b200ldu_solve(b200ldu_matrix *m, const char *solver, const char *pre,
