@@ -20,12 +20,15 @@ sys.path.insert(0, ROOT)
 
 def pcg_sweep_bytes(info):
     """Bytes the banded layout moves in the two sweeps of one fused PCG iteration (single domain: every entry is
-    local).  Stream: the face stream's stored owner slots and list items, 8 B coefficient + 4 B column and product
-    slot each, or, for a layout without one, the entry stream's 8 B coefficient + 2 B column per entry.  Halo: a
-    4 B haloIdx per column plus the vectors the op's stage() reads there.  Own rows: the vectors read and written
-    while staging and in finish()."""
+    local).  Stream: the face stream's stored owner slots and list items, an 8 B coefficient each, plus its table of
+    4 B column and product-slot words once, or, for a layout without one, the entry stream's 8 B coefficient + 2 B
+    column per entry.  Halo: a 4 B haloIdx per column plus the vectors the op's stage() reads there.  Own rows: the
+    vectors read and written while staging and in finish()."""
     nPad, nE, nH = info["nPadRows"], info["nEntries"], info["nHalo"]
-    stream = 12 * (info["fsOwnerSlots"] + info["fsListItems"]) if info.get("faceStream") else 10 * nE
+    if info.get("faceStream"):
+        stream = 8 * (info["fsOwnerSlots"] + info["fsListItems"]) + 4 * info["fsTemplateWords"]
+    else:
+        stream = 10 * nE
     # A (PcgAinvOp): own rows read rOld, w, rD and write rNew, z; halo reads w, rOld, rD
     a = 40 * nPad + stream + (4 + 24) * nH
     # B (PcgAmulOp): own rows read z, pOld, psi, diag and write pNew, psi, w; halo reads z, pOld

@@ -118,6 +118,9 @@ int b200ldu_addr_info(const b200ldu_addr *a, long long *nPadRows, long long *nEn
  * of the largest band, and whether symmetric matrices on this addressing use it (1) or the entry stream (0) */
 int b200ldu_addr_face_info(const b200ldu_addr *a, long long *nOwnerSlots, long long *nListItems, int *bufDoubles,
                            int *used);
+/* the face stream's table of distinct column and product-slot blocks (one per repeated slice or band list): its
+ * 32-bit words and its blocks; 0 and 0 where symmetric matrices use the entry stream */
+int b200ldu_addr_face_templates(const b200ldu_addr *a, long long *words, int *count);
 /* cell renumbering: perm_h[c] = banded row of caller cell c (HOST int32[nCells]) */
 int b200ldu_addr_perm(const b200ldu_addr *a, int *perm_h);
 

@@ -52,7 +52,8 @@ class Perf(C.Structure):
 EXPORTS = [
     "b200ldu_last_error", "b200ldu_controls_default", "b200ldu_ctx_create", "b200ldu_ctx_destroy",
     "b200ldu_comm_unique_id", "b200ldu_comm_init", "b200ldu_comm_info", "b200ldu_ctx_set_stream", "b200ldu_ctx_sync",
-    "b200ldu_addr_create", "b200ldu_addr_destroy", "b200ldu_addr_info", "b200ldu_addr_face_info", "b200ldu_addr_perm",
+    "b200ldu_addr_create", "b200ldu_addr_destroy", "b200ldu_addr_info", "b200ldu_addr_face_info",
+    "b200ldu_addr_face_templates", "b200ldu_addr_perm",
     "b200ldu_matrix_create", "b200ldu_matrix_set", "b200ldu_matrix_destroy",
     "b200ldu_amul", "b200ldu_tmul", "b200ldu_sumA", "b200ldu_residual", "b200ldu_H", "b200ldu_H1",
     "b200ldu_faceH", "b200ldu_precondition", "b200ldu_smooth",
@@ -106,6 +107,7 @@ def lib():
                                     C.POINTER(C.c_longlong), C.POINTER(C.c_int), C.POINTER(C.c_int)]
     L.b200ldu_addr_face_info.argtypes = [vp, C.POINTER(C.c_longlong), C.POINTER(C.c_longlong), C.POINTER(C.c_int),
                                          C.POINTER(C.c_int)]
+    L.b200ldu_addr_face_templates.argtypes = [vp, C.POINTER(C.c_longlong), C.POINTER(C.c_int)]
     L.b200ldu_addr_perm.argtypes = [vp, vp]
     L.b200ldu_matrix_create.argtypes = [vp, C.POINTER(vp)]
     L.b200ldu_matrix_set.argtypes = [vp, vp, vp, vp, vp, vp]
@@ -268,8 +270,11 @@ class LduAddressing:
         check(lib().b200ldu_addr_info(self.h, C.byref(a), C.byref(b), C.byref(c), C.byref(d), C.byref(e)))
         fo, fl, fb, fu = C.c_longlong(), C.c_longlong(), C.c_int(), C.c_int()
         check(lib().b200ldu_addr_face_info(self.h, C.byref(fo), C.byref(fl), C.byref(fb), C.byref(fu)))
+        tw, tc = C.c_longlong(), C.c_int()
+        check(lib().b200ldu_addr_face_templates(self.h, C.byref(tw), C.byref(tc)))
         return dict(nPadRows=a.value, nEntries=b.value, nHalo=c.value, bandRows=d.value, nBands=e.value,
-                    fsOwnerSlots=fo.value, fsListItems=fl.value, fsBufDoubles=fb.value, faceStream=bool(fu.value))
+                    fsOwnerSlots=fo.value, fsListItems=fl.value, fsBufDoubles=fb.value, faceStream=bool(fu.value),
+                    fsTemplateWords=tw.value, fsTemplates=tc.value)
 
     def perm(self):
         p = np.zeros(self.nCells, dtype=np.int32)

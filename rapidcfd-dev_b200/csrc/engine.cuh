@@ -113,7 +113,8 @@ __device__ __forceinline__ void block_reduce_store(double (&red)[NRED], double *
 //                                writes rows r, r+1; adds reductions
 //
 // Face stream (FS, symmetric matrices; layout.cu): the band's product buffer follows the tile in shared memory and
-// starts filled with identity().  Pass 1 streams the owner slots of each row: add(init, owner terms) in face order,
+// starts filled with identity().  Pass 1 streams the owner slots of each row (the coefficients from HBM, their column and
+// product-slot words from the layout's template table, which stays in L1 and L2): add(init, owner terms) in face order,
 // stored in the row's slot 0, while every owner entry whose neighbour row lies in the band stores prod(v, a_own) in
 // that row's neighbour slot; the CTA then stores the products of the band's list (faces owned in other bands,
 // coupled-patch faces).  After one barrier pass 2 adds each row's slots in order -- neighbour faces in losort order,
@@ -128,10 +129,11 @@ __host__ __device__ __forceinline__ bool fused_pack(const Op &op, const LayoutDe
     return Op::STAGED && !Op::LOCAL && op.waitHalo && L.nPackChunks > 0;
 }
 
-__device__ __forceinline__ uint2 ldg_stream_u64(const void *p)
+// the face stream's words come from a small table that many slices share: keep them in L1
+__device__ __forceinline__ uint2 ldg_table_u64(const void *p)
 {
     uint2 r;
-    asm volatile("ld.global.nc.L1::no_allocate.v2.u32 {%0, %1}, [%2];" : "=r"(r.x), "=r"(r.y) : "l"(p));
+    asm volatile("ld.global.nc.v2.u32 {%0, %1}, [%2];" : "=r"(r.x), "=r"(r.y) : "l"(p));
     return r;
 }
 
@@ -230,18 +232,17 @@ __global__ void __launch_bounds__(ENGINE_THREADS, 6) engine_kernel(const LayoutD
             const double a0 = Op::STAGED ? xs[lr] : 0, a1 = Op::STAGED ? xs[lr + 1] : 0;
             double acc0 = op.init(rowBase + lr, a0);
             double acc1 = op.init(rowBase + lr + 1, a1);
-            const long long base = (long long)S.start64 * SLICE_ROWS + 2 * lane;
-            const double *vp = val + base;
-            const uint32_t *cp = L.fsCT + base;
-            const int W = S.wo;
-            int j = 0;
-            for (; j + 4 <= W; j += 4) {
+            // 32-bit offsets of the lane's first slot, advanced slot by slot: the layout keeps the coefficient stream and
+            // the template table below 2^31 entries (fsFits)
+            unsigned vo = S.start64 * SLICE_ROWS + 2 * lane, co = S.tpl64 * SLICE_ROWS + 2 * lane;
+            int n = S.wo;
+            for (; n >= 4; n -= 4, vo += 4 * SLICE_ROWS, co += 4 * SLICE_ROWS) {
                 double2 v[4];
                 uint2 c[4];
 #pragma unroll
                 for (int k = 0; k < 4; k++) {
-                    v[k] = ldg_stream2(vp + (size_t)(j + k) * SLICE_ROWS);
-                    c[k] = ldg_stream_u64(cp + (size_t)(j + k) * SLICE_ROWS);
+                    v[k] = ldg_stream2(val + (vo + k * SLICE_ROWS));
+                    c[k] = ldg_table_u64(L.fsTpl + (co + k * SLICE_ROWS));
                 }
 #pragma unroll
                 for (int k = 0; k < 4; k++) {
@@ -249,19 +250,20 @@ __global__ void __launch_bounds__(ENGINE_THREADS, 6) engine_kernel(const LayoutD
                     acc1 = fs_owner(op, xs, buf, acc1, v[k].y, c[k].y, a1);
                 }
             }
-            for (; j < W; j++) {
-                double2 v = ldg_stream2(vp + (size_t)j * SLICE_ROWS);
-                uint2 c = ldg_stream_u64(cp + (size_t)j * SLICE_ROWS);
+            for (; n > 0; n--, vo += SLICE_ROWS, co += SLICE_ROWS) {
+                double2 v = ldg_stream2(val + vo);
+                uint2 c = ldg_table_u64(L.fsTpl + co);
                 acc0 = fs_owner(op, xs, buf, acc0, v.x, c.x, a0);
                 acc1 = fs_owner(op, xs, buf, acc1, v.y, c.y, a1);
             }
             reinterpret_cast<double2 *>(buf + S.bufOff)[lane] = make_double2(acc0, acc1);
         }
         {
-            const int le = Op::LOCAL ? L.fsListIfc[band] : L.fsListStart[band + 1];
-            for (int i = L.fsListStart[band] + tid; i < le; i += ENGINE_THREADS) {
+            const int ls = L.fsListStart[band], le = Op::LOCAL ? L.fsListIfc[band] : L.fsListStart[band + 1];
+            const int tpl = L.fsListTpl[band] - ls; // list item i's word is fsTpl[tpl + i]
+            for (int i = ls + tid; i < le; i += ENGINE_THREADS) {
                 const double v = __ldcs(val + i);
-                const uint32_t ct = __ldcs(L.fsCT + i);
+                const uint32_t ct = __ldg(L.fsTpl + (tpl + i));
                 buf[ct >> 16] = op.prod(v, Op::STAGED ? xs[ct & 0xffffu] : 0);
             }
         }

@@ -183,12 +183,13 @@ struct PackChunk {
 // Face stream of a symmetric matrix (layout.cu, engine.cuh): every face is stored once, in its owner's row; the
 // product for the neighbour's row goes through a per-band shared-memory buffer.  Per slice of 64 rows:
 struct FsSlice {
-    int start64;      // owner-stream offset of the slice / 64
-    int bufOff;       // offset of the slice's product slots in the band's buffer (doubles)
+    int start64;      // owner-stream offset of the slice's coefficients / 64
+    int tpl64;        // offset of the slice's column and product-slot words in the template table / 64
+    uint16_t bufOff;  // offset of the slice's product slots in the band's buffer (doubles; < FS_PAD)
     uint16_t wo;      // owner slots per row
     uint16_t wn, wi;  // buffer slots per row after slot 0 (the owner-pass sum): neighbour faces, then interface faces
-    uint16_t unused;
 };
+static_assert(sizeof(FsSlice) == 16, "one 128-bit load per slice");
 // 16-bit product-slot value of an owner entry: a buffer index, or one of these
 constexpr uint32_t FS_PAD = 0xfffe;  // padding entry: contributes nothing
 constexpr uint32_t FS_NONE = 0xffff; // the neighbour row lies in another band (its band's list carries the product)
@@ -208,10 +209,13 @@ struct LayoutDev {
     const uint16_t *col;         // [nEntries] band-local column: < bandRows own band, else halo slot
     const int *haloStart;        // [nBands+1]
     const int *haloIdx;          // banded extended index: < nPad local row, else nPad + recv slot
-    // face stream (null when the layout has none): entries [0, nOwn) are the slot-major owner stream, then the
-    // per-band lists; each entry's word is column | product slot << 16
+    // face stream (null when the layout has none): coefficients [0, nOwn) are the slot-major owner stream, then the
+    // per-band lists.  Each entry's word, column | product slot << 16, depends on the mesh and the layout alone and is
+    // read from a table of distinct blocks: a slice's owner words at fsTpl + 64 tpl64 (slot-major, wo x 64 words), a
+    // band's list words at fsTpl + fsListTpl[b]
     const FsSlice *fsSlice;      // [nSlices]
-    const uint32_t *fsCT;        // [nOwn + nList]
+    const uint32_t *fsTpl;       // template table
+    const int *fsListTpl;        // [nBands]
     const int *fsListStart;      // [nBands+1] list of band b: [fsListStart[b], fsListIfc[b]) faces whose owner row
     const int *fsListIfc;        // [nBands]   lies in another band, then coupled-patch faces up to fsListStart[b+1]
     int fsBufMax;                // product-buffer doubles of the largest band
@@ -248,8 +252,9 @@ struct LayoutHost {
     std::vector<int> sendRows; // [nRecv] banded row of faceCells
     // face stream (empty where it was not built)
     std::vector<FsSlice> fsSlice;
-    std::vector<uint32_t> fsCT;
-    std::vector<int> fsCode, fsListStart, fsListIfc;
+    std::vector<uint32_t> fsTpl; // template table of the column and product-slot words
+    int fsTplCount = 0;          // distinct blocks in it
+    std::vector<int> fsListTpl, fsCode, fsListStart, fsListIfc;
 };
 
 // slots of b200ldu_addr::mem
@@ -280,6 +285,8 @@ struct b200ldu_addr {
     // face stream: used by symmetric matrices when the layout has one (hasFs)
     bool hasFs = false;
     long long fsOwn = 0, fsList = 0; // stored owner slots (padding included), list items
+    long long fsTplWords = 0;        // template table: words, distinct blocks
+    int fsTplCount = 0;
     int *d_fsCode = nullptr; // [fsOwn + fsList] value source, as d_code
     bool p2pHalo = false;      // peer-store halo usable for this addressing
     double nCellsGlobal = 0;

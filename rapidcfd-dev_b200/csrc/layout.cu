@@ -18,12 +18,13 @@
 //
 // layout_build runs in stages: addressing checks and CSR, renumbering, coupled-patch face
 // lists, then a plan for a band size (halved until the band fits), the face-stream choice,
-// and the fills of the entry stream and (where it is used) the face stream.
+// and the fills of the entry stream and (where it is used) the face stream and its template table.
 #include <algorithm>
 #include <cmath>
 #include <cstdlib>
 #include <numeric>
 #include <queue>
+#include <unordered_map>
 
 #include "internal.h"
 
@@ -315,7 +316,7 @@ int plan_layout(const Graph &g, const std::vector<int> &order, const std::vector
         if (wl + wi > 65535) bad++;
         H.sliceWL[s] = (uint16_t)wl;
         H.sliceW[s] = (uint16_t)(wl + wi);
-        H.fsSlice[s] = FsSlice{0, 0, (uint16_t)wo, (uint16_t)wn, (uint16_t)wi, 0};
+        H.fsSlice[s] = FsSlice{0, 0, 0, (uint16_t)wo, (uint16_t)wn, (uint16_t)wi};
     }
     if (bad) {
         b200_set_error("layout_build: a row has more than 65535 entries");
@@ -333,7 +334,7 @@ int plan_layout(const Graph &g, const std::vector<int> &order, const std::vector
         for (int sl = 0; sl < slicesPerBand; sl++) {
             FsSlice &S = H.fsSlice[(size_t)b * slicesPerBand + sl];
             S.start64 = (int)(fsOwn / SLICE_ROWS);
-            S.bufOff = (int)std::min<long long>(off, INT32_MAX);
+            S.bufOff = (uint16_t)std::min<long long>(off, 0xffff); // exact where the face stream fits (fsFits)
             fsOwn += (long long)S.wo * SLICE_ROWS;
             off += (1 + (long long)S.wn + S.wi) * SLICE_ROWS;
         }
@@ -486,7 +487,8 @@ void fill_entry_stream(const Graph &g, const std::vector<int> &perm, Plan &P)
 }
 
 // ---- 7. face stream: owner entries, then each band's list ---------------------------
-void fill_face_stream(const Graph &g, const std::vector<int> &perm, Plan &P)
+// fsCT[i]: the column and product-slot word of face-stream entry i (templates are made of them below)
+void fill_face_stream(const Graph &g, const std::vector<int> &perm, Plan &P, std::vector<uint32_t> &fsCT)
 {
     LayoutHost &H = P.H;
     const int bandRows = H.bandRows, slicesPerBand = bandRows / SLICE_ROWS, nPad = H.nPad;
@@ -495,7 +497,6 @@ void fill_face_stream(const Graph &g, const std::vector<int> &perm, Plan &P)
     std::vector<int> nbSlot((size_t)std::max(g.nFaces, 1));
     for (int c = 0; c < g.nCells; c++)
         for (int k = g.losortStart[c]; k < g.losortStart[c + 1]; k++) nbSlot[g.losort[k]] = k - g.losortStart[c];
-    std::vector<uint32_t> &fsCT = H.fsCT;
     std::vector<int> &fsCode = H.fsCode;
     fsCT.assign((size_t)std::max<long long>(H.fsOwn + H.fsList, 1), 0);
     fsCode.assign(fsCT.size(), 0);
@@ -547,7 +548,78 @@ void fill_face_stream(const Graph &g, const std::vector<int> &perm, Plan &P)
     }
 }
 
-// ---- 8. device path: upload the record into fixed arrays of the addressing, set every layout field of it ----
+// ---- 8. face-stream templates ---------------------------------------------------------
+// The words depend on the mesh topology and the layout, not on the matrix, and on a structured mesh the slices and
+// bands of the interior repeat (256^3 in 512-row bands: 163 distinct slices of 262144, 16 distinct band lists of
+// 32768).  Every slice's owner block (wo x 64 words) and every band's list block becomes a reference into one table
+// of distinct blocks, so that a sweep streams only the coefficients from HBM and reads the words from a table that
+// stays in L2 and L1.  Owner blocks come first, so their offsets are multiples of 64; a new block is appended in
+// slice order, then band order, whatever the number of threads that hashed them.
+void build_face_templates(const std::vector<uint32_t> &fsCT, LayoutHost &H)
+{
+    const int nSlices = (int)H.fsSlice.size(), nBlocks = nSlices + H.nBands;
+    auto block = [&](int k, long long &begin, long long &n) {
+        if (k < nSlices) {
+            begin = (long long)H.fsSlice[k].start64 * SLICE_ROWS;
+            n = (long long)H.fsSlice[k].wo * SLICE_ROWS;
+        } else {
+            begin = H.fsListStart[k - nSlices];
+            n = H.fsListStart[k - nSlices + 1] - begin;
+        }
+    };
+    std::vector<uint64_t> hash(nBlocks);
+#pragma omp parallel for schedule(dynamic, 64)
+    for (int k = 0; k < nBlocks; k++) {
+        long long begin, n;
+        block(k, begin, n);
+        uint64_t h = 0x9e3779b97f4a7c15ull ^ (uint64_t)n;
+        for (long long i = 0; i < n; i++) {
+            h = (h ^ fsCT[begin + i]) * 0xff51afd7ed558ccdull;
+            h ^= h >> 29;
+        }
+        hash[k] = h;
+    }
+    std::unordered_map<uint64_t, std::vector<std::pair<long long, long long>>> seen; // hash -> (offset, words)
+    std::vector<uint32_t> &tpl = H.fsTpl;
+    tpl.clear();
+    H.fsTplCount = 0;
+    H.fsListTpl.assign(H.nBands, 0);
+    for (int k = 0; k < nBlocks; k++) {
+        long long begin, n, off = -1;
+        block(k, begin, n);
+        std::vector<std::pair<long long, long long>> &cand = seen[hash[k]];
+        for (const auto &t : cand)
+            if (t.second == n && std::equal(fsCT.begin() + begin, fsCT.begin() + begin + n, tpl.begin() + t.first)) {
+                off = t.first;
+                break;
+            }
+        if (off < 0) {
+            off = (long long)tpl.size();
+            tpl.insert(tpl.end(), fsCT.begin() + begin, fsCT.begin() + begin + n);
+            cand.emplace_back(off, n);
+            H.fsTplCount++;
+        }
+        if (k < nSlices)
+            H.fsSlice[k].tpl64 = (int)(off / SLICE_ROWS);
+        else
+            H.fsListTpl[k - nSlices] = (int)off;
+    }
+}
+
+// every face-stream entry's word, expanded from the templates: what the table stands for
+std::vector<uint32_t> face_words(const LayoutHost &H)
+{
+    std::vector<uint32_t> ct((size_t)(H.fsOwn + H.fsList));
+    for (const FsSlice &S : H.fsSlice)
+        std::copy_n(H.fsTpl.begin() + (long long)S.tpl64 * SLICE_ROWS, (long long)S.wo * SLICE_ROWS,
+                    ct.begin() + (long long)S.start64 * SLICE_ROWS);
+    for (int b = 0; b < H.nBands; b++)
+        std::copy_n(H.fsTpl.begin() + H.fsListTpl[b], H.fsListStart[b + 1] - H.fsListStart[b],
+                    ct.begin() + H.fsListStart[b]);
+    return ct;
+}
+
+// ---- 9. device path: upload the record into fixed arrays of the addressing, set every layout field of it ----
 int layout_upload(b200ldu_addr *a, const Graph &g, const LayoutHost &H)
 {
     LayoutDev &L = a->L;
@@ -569,7 +641,8 @@ int layout_upload(b200ldu_addr *a, const Graph &g, const LayoutHost &H)
     TRY(mem.upload(a->d_losortStart, g.losortStart));
     if (H.hasFs) {
         TRY(mem.upload(L.fsSlice, H.fsSlice));
-        TRY(mem.upload(L.fsCT, H.fsCT));
+        TRY(mem.upload(L.fsTpl, H.fsTpl));
+        TRY(mem.upload(L.fsListTpl, H.fsListTpl));
         TRY(mem.upload(a->d_fsCode, H.fsCode));
         TRY(mem.upload(L.fsListStart, H.fsListStart));
         TRY(mem.upload(L.fsListIfc, H.fsListIfc));
@@ -588,6 +661,8 @@ int layout_upload(b200ldu_addr *a, const Graph &g, const LayoutHost &H)
     a->hasFs = H.hasFs;
     a->fsOwn = H.fsOwn;
     a->fsList = H.fsList;
+    a->fsTplWords = (long long)H.fsTpl.size();
+    a->fsTplCount = H.fsTplCount;
     return B200LDU_OK;
 }
 
@@ -626,7 +701,9 @@ int layout_build(b200ldu_addr *a, const double *centres)
     fill_entry_stream(g, a->perm_h, P);
     // a host-only layout keeps the face stream whether or not the engine would use it, so that its structure can be checked
     if (P.fsFits && (H.hasFs || a->hostOnly)) {
-        fill_face_stream(g, a->perm_h, P);
+        std::vector<uint32_t> fsCT;
+        fill_face_stream(g, a->perm_h, P, fsCT);
+        build_face_templates(fsCT, H);
     } else { // the record holds a face stream only where it was built
         H.fsSlice.clear();
         H.fsListStart.clear();
@@ -674,8 +751,9 @@ extern "C" int b200ldu_layout_debug_create(int nCells, int nFaces, const int *lo
 // what: 0 perm(int32) 1 iperm(int32) 2 sliceStart(int64) 3 sliceW(u16) 4 sliceWL(u16) 5 col(u16)
 //       6 code(int32) 7 haloStart(int32) 8 haloIdx(int32) 9 dims {nPad,nBands,bandRows,nRecv,maxHalo}(int32)
 //       face stream (empty when it was not built): 10 fsSlice (4 int32 per slice: start64, bufOff, wo | wn << 16,
-//       wi) 11 fsCT(u32) 12 fsCode(int32) 13 fsListStart(int32) 14 fsListIfc(int32)
-//       15 fs dims {fsOwn, fsList, fsBufMax, hasFs}(int64)
+//       wi) 11 column and product-slot word of every entry, expanded from the templates (u32) 12 fsCode(int32)
+//       13 fsListStart(int32) 14 fsListIfc(int32) 15 fs dims {fsOwn, fsList, fsBufMax, hasFs}(int64)
+//       16 template table fsTpl(u32) 17 tpl64 of every slice(int32) 18 fsListTpl(int32)
 // returns the element count (copies min(count, cap) elements when out != NULL)
 extern "C" long long b200ldu_layout_debug_get(const b200ldu_addr *a, int what, void *out, long long cap)
 {
@@ -685,8 +763,9 @@ extern "C" long long b200ldu_layout_debug_get(const b200ldu_addr *a, int what, v
         if (out) memcpy(out, src, elem * (size_t)std::min(n, cap));
         return n;
     };
-    const long long nFs = H.fsCT.empty() ? 0 : H.fsOwn + H.fsList;
+    const long long nFs = H.fsSlice.empty() ? 0 : H.fsOwn + H.fsList;
     int dims[5] = {H.nPad, H.nBands, H.bandRows, H.nRecv, H.maxHalo};
+    std::vector<int> perSlice;
     switch (what) {
     case 0: return give(a->perm_h.data(), 4, (long long)a->perm_h.size());
     case 1: return give(a->iperm_h.data(), 4, (long long)a->iperm_h.size());
@@ -698,8 +777,14 @@ extern "C" long long b200ldu_layout_debug_get(const b200ldu_addr *a, int what, v
     case 7: return give(H.haloStart.data(), 4, (long long)H.haloStart.size());
     case 8: return give(H.haloIdx.data(), 4, H.haloStart[H.nBands]);
     case 9: return give(dims, 4, 5);
-    case 10: return give(H.fsSlice.data(), 4, 4 * (long long)H.fsSlice.size());
-    case 11: return give(H.fsCT.data(), 4, nFs);
+    case 10:
+        for (const FsSlice &S : H.fsSlice)
+            perSlice.insert(perSlice.end(), {S.start64, (int)S.bufOff, S.wo | S.wn << 16, (int)S.wi});
+        return give(perSlice.data(), 4, (long long)perSlice.size());
+    case 11: {
+        const std::vector<uint32_t> ct = nFs ? face_words(H) : std::vector<uint32_t>();
+        return give(ct.data(), 4, nFs);
+    }
     case 12: return give(H.fsCode.data(), 4, nFs);
     case 13: return give(H.fsListStart.data(), 4, (long long)H.fsListStart.size());
     case 14: return give(H.fsListIfc.data(), 4, (long long)H.fsListIfc.size());
@@ -707,6 +792,11 @@ extern "C" long long b200ldu_layout_debug_get(const b200ldu_addr *a, int what, v
         long long fd[4] = {H.fsOwn, H.fsList, (int)H.fsBufMax, H.hasFs ? 1 : 0};
         return give(fd, 8, 4);
     }
+    case 16: return give(H.fsTpl.data(), 4, (long long)H.fsTpl.size());
+    case 17:
+        for (const FsSlice &S : H.fsSlice) perSlice.push_back(S.tpl64);
+        return give(perSlice.data(), 4, (long long)perSlice.size());
+    case 18: return give(H.fsListTpl.data(), 4, (long long)H.fsListTpl.size());
     }
     return -1;
 }

@@ -211,6 +211,14 @@ extern "C" int b200ldu_addr_face_info(const b200ldu_addr *a, long long *nOwnerSl
     return B200LDU_OK;
 }
 
+extern "C" int b200ldu_addr_face_templates(const b200ldu_addr *a, long long *words, int *count)
+{
+    if (!a) return B200LDU_EINVAL;
+    if (words) *words = a->fsTplWords;
+    if (count) *count = a->fsTplCount;
+    return B200LDU_OK;
+}
+
 extern "C" int b200ldu_addr_perm(const b200ldu_addr *a, int *perm_h)
 {
     if (!a || !perm_h) return B200LDU_EINVAL;
