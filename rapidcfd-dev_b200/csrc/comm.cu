@@ -298,15 +298,10 @@ int comm_halo_exchange(b200ldu_addr *a, double *x, double *sendBuf, const int *s
     bool remote = false;
     for (int p = 0; p < a->nPatches; p++)
         if (a->neighbRank[p] >= 0) remote = true;
-    if (a->d_cyclicSrc) { // cyclic partners: x[nPad + face] = x[partner's face cell]
-        cyclic_fill_kernel<<<(nRecv + 255) / 256, 256, 0, ctx->stream>>>(nRecv, a->d_cyclicSrc, x, x + a->L.nPad, stop);
-        ctx->launches++;
-        KERNEL_CHECK();
-    }
+    if (a->d_cyclicSrc) // cyclic partners: x[nPad + face] = x[partner's face cell]
+        TRY(launch(ctx, cyclic_fill_kernel, nRecv, 256, nRecv, a->d_cyclicSrc, x, x + a->L.nPad, stop));
     if (!remote) return B200LDU_OK;
-    pack_kernel<<<(nRecv + 255) / 256, 256, 0, ctx->stream>>>(nRecv, a->L.sendRows, x, sendBuf, stop);
-    ctx->launches++;
-    KERNEL_CHECK();
+    TRY(launch(ctx, pack_kernel, nRecv, 256, nRecv, a->L.sendRows, x, sendBuf, stop));
     if (remote && !ctx->nccl) {
         b200_set_error("halo exchange: processor patches present but no communicator (b200ldu_comm_init)");
         return B200LDU_ENCCL;

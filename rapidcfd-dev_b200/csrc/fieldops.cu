@@ -19,73 +19,47 @@ extern "C" int b200ldu_field_binary(b200ldu_ctx *ctx, int op, long long n, int n
 {
     if (!ctx || !a_d || !b_d || !out_d || n < 0 || op < OP_ADD || op > OP_MAX) return B200LDU_EINVAL;
     if ((ncA != 1 && ncA != 3) || (ncB != 1 && ncB != 3)) return B200LDU_EINVAL;
-    if (n == 0) return B200LDU_OK;
     CUDA_TRY(cudaSetDevice(ctx->device));
     const int nc = ncA > ncB ? ncA : ncB;
-    const long long tot = n * nc;
-    binary_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, ctx->stream>>>(n, nc, ncA, ncB, op, a_d, b_d, out_d);
-    ctx->launches++;
-    KERNEL_CHECK();
-    return B200LDU_OK;
+    return launch(ctx, binary_kernel, n * nc, 256, n, nc, ncA, ncB, op, a_d, b_d, out_d);
 }
 
 extern "C" int b200ldu_field_unary(b200ldu_ctx *ctx, int op, long long n, double s, const double *a_d, double *out_d)
 {
     if (!ctx || !a_d || !out_d || n < 0 || op < UN_NEG || op > UN_POS) return B200LDU_EINVAL;
-    if (n == 0) return B200LDU_OK;
     CUDA_TRY(cudaSetDevice(ctx->device));
-    unary_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(n, op, s, a_d, out_d);
-    ctx->launches++;
-    KERNEL_CHECK();
-    return B200LDU_OK;
+    return launch(ctx, unary_kernel, n, 256, n, op, s, a_d, out_d);
 }
 
 extern "C" int b200ldu_field_dot3(b200ldu_ctx *ctx, long long n, const double *a_d, const double *b_d, double *out_d)
 {
     if (!ctx || !a_d || !b_d || !out_d || n < 0) return B200LDU_EINVAL;
-    if (n == 0) return B200LDU_OK;
     CUDA_TRY(cudaSetDevice(ctx->device));
-    dot3_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(n, a_d, b_d, out_d);
-    ctx->launches++;
-    KERNEL_CHECK();
-    return B200LDU_OK;
+    return launch(ctx, dot3_kernel, n, 256, n, a_d, b_d, out_d);
 }
 
 extern "C" int b200ldu_field_symm_magsqr(b200ldu_ctx *ctx, long long n, const double *tensor_d, double *out_d)
 {
     if (!ctx || !tensor_d || !out_d || n < 0) return B200LDU_EINVAL;
-    if (n == 0) return B200LDU_OK;
     CUDA_TRY(cudaSetDevice(ctx->device));
-    symm_magsqr_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(n, tensor_d, out_d);
-    ctx->launches++;
-    KERNEL_CHECK();
-    return B200LDU_OK;
+    return launch(ctx, symm_magsqr_kernel, n, 256, n, tensor_d, out_d);
 }
 
 extern "C" int b200ldu_field_gather(b200ldu_ctx *ctx, int n, int nComp, const int *cells_d, const double *field_d,
                                     double *out_d)
 {
     if (!ctx || !cells_d || !field_d || !out_d || n < 0 || (nComp != 1 && nComp != 3)) return B200LDU_EINVAL;
-    if (n == 0) return B200LDU_OK;
     CUDA_TRY(cudaSetDevice(ctx->device));
-    gather_kernel<<<(unsigned)(((long long)n * nComp + 255) / 256), 256, 0, ctx->stream>>>(n, nComp, cells_d, field_d, out_d);
-    ctx->launches++;
-    KERNEL_CHECK();
-    return B200LDU_OK;
+    return launch(ctx, gather_kernel, (long long)n * nComp, 256, n, nComp, cells_d, field_d, out_d);
 }
 
 // snGradScheme::snGrad of a cell field on the internal faces (the boundary values come from the boundary conditions)
 extern "C" int b200ldu_fv_sngrad(b200ldu_addr *a, int nComp, const double *deltaCoeffs_d, const double *vf_d, double *out_d)
 {
     if (!a || !deltaCoeffs_d || !vf_d || !out_d || (nComp != 1 && nComp != 3)) return B200LDU_EINVAL;
-    if (a->nFaces == 0) return B200LDU_OK;
     CUDA_TRY(cudaSetDevice(a->ctx->device));
-    const long long tot = (long long)a->nFaces * nComp;
-    sngrad_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, a->ctx->stream>>>(a->nFaces, nComp, a->d_l, a->d_u, deltaCoeffs_d, vf_d,
-                                                                             out_d);
-    a->ctx->launches++;
-    KERNEL_CHECK();
-    return B200LDU_OK;
+    return launch(a->ctx, sngrad_kernel, (long long)a->nFaces * nComp, 256, a->nFaces, nComp, a->d_l, a->d_u, deltaCoeffs_d,
+                  vf_d, out_d);
 }
 
 // ---- limited / upwind interpolation weights (SURVEY.md section 8(f) rank 1) ----
@@ -115,14 +89,10 @@ extern "C" int b200ldu_fv_limiter(b200ldu_addr *a, const char *scheme, double k,
         b200_set_error("limitedLinear: coefficient = %g should be >= 0 and <= 1 (limitedLinear.H:66-72)", k);
         return B200LDU_EINVAL;
     }
-    if (a->nFaces == 0) return B200LDU_OK;
     CUDA_TRY(cudaSetDevice(a->ctx->device));
     const double kk = k > 1e-15 ? k : 1e-15;   // twoByk_ = 2.0/max(k_, SMALL), SMALL = 1e-15 (doubleScalar.H)
-    limiter_kernel<<<(a->nFaces + 255) / 256, 256, 0, a->ctx->stream>>>(a->nFaces, sch, 2.0 / kk, a->d_l, a->d_u, faceFlux_d, vf_d,
-                                                                       gradc_d, C_d, limiter_d);
-    a->ctx->launches++;
-    KERNEL_CHECK();
-    return B200LDU_OK;
+    return launch(a->ctx, limiter_kernel, a->nFaces, 256, a->nFaces, sch, 2.0 / kk, a->d_l, a->d_u, faceFlux_d, vf_d, gradc_d,
+                  C_d, limiter_d);
 }
 
 // weights of a limited scheme from its limiter field (limitedSurfaceInterpolationScheme.C:155-212); limiter_d NULL: upwind
@@ -131,10 +101,6 @@ extern "C" int b200ldu_fv_limited_weights(b200ldu_ctx *ctx, long long n, const d
                                           const double *faceFlux_d, double *weights_d)
 {
     if (!ctx || !faceFlux_d || !weights_d || n < 0 || (limiter_d && !cdWeights_d)) return B200LDU_EINVAL;
-    if (n == 0) return B200LDU_OK;
     CUDA_TRY(cudaSetDevice(ctx->device));
-    limited_weights_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(n, limiter_d, cdWeights_d, faceFlux_d, weights_d);
-    ctx->launches++;
-    KERNEL_CHECK();
-    return B200LDU_OK;
+    return launch(ctx, limited_weights_kernel, n, 256, n, limiter_d, cdWeights_d, faceFlux_d, weights_d);
 }

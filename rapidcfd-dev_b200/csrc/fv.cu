@@ -13,13 +13,12 @@
 // written once (the reference runs one kernel per patch plus a separate divide).
 // Summation order = owner faces, neighbour faces, boundary faces (ascending), then /V,
 // products rounded separately -- bit-comparable with oracle/ldu_oracle_fv.c.
-#include <algorithm>
-
 #include "internal.h"
 
 #include "fv_kernels.cuh"
 
 using namespace fvk;
+using fvmk::BoundaryLists;
 
 extern "C" int b200ldu_fv_boundary_set(b200ldu_addr *a, int nBFaces, const int *bFaceCells_h)
 {
@@ -31,14 +30,8 @@ extern "C" int b200ldu_fv_boundary_set(b200ldu_addr *a, int nBFaces, const int *
             return B200LDU_EINVAL;
         }
     // per cell CSR over boundary faces, ascending boundary-face index inside a cell
-    std::vector<int> start((size_t)a->nCells + 1, 0), faces(std::max(nBFaces, 1));
-    for (int i = 0; i < nBFaces; i++) start[bFaceCells_h[i] + 1]++;
-    for (int c = 0; c < a->nCells; c++) start[c + 1] += start[c];
-    {
-        std::vector<int> cur(start.begin(), start.end() - 1);
-        for (int i = 0; i < nBFaces; i++) faces[cur[bFaceCells_h[i]]++] = i;
-    }
-    std::vector<int> fc(bFaceCells_h, bFaceCells_h + nBFaces);
+    std::vector<int> fc(bFaceCells_h, bFaceCells_h + nBFaces), start, faces;
+    csr_from_map(fc, a->nCells, start, faces);
     // the lists are rewritten in place: work still queued may read the old ones, and until all three are written the
     // addressing has no boundary list (an upload that fails leaves it so)
     CUDA_TRY(cudaStreamSynchronize(a->ctx->stream));
@@ -57,19 +50,11 @@ extern "C" int b200ldu_fv_surface_integrate(b200ldu_addr *a, int nComp, const do
     if (!a || !ssf_d || !out_d || (divideByV && !V_d) || (nComp != 1 && nComp != 3)) return B200LDU_EINVAL;
     if (a->nBFaces && !bssf_d) return B200LDU_EINVAL;
     CUDA_TRY(cudaSetDevice(a->ctx->device));
-    const int *bs = a->nBFaces ? a->d_bCellStart : nullptr;
-    dim3 g((a->nCells + 127) / 128), b(128);
-    if (nComp == 1)
-        surface_integrate_kernel<1><<<g, b, 0, a->ctx->stream>>>(a->nCells, a->d_ownerStart, a->d_losortStart,
-                                                                  a->d_losort, bs, a->d_bCellFaces, ssf_d, bssf_d,
-                                                                  V_d, out_d, divideByV, neiSign);
-    else
-        surface_integrate_kernel<3><<<g, b, 0, a->ctx->stream>>>(a->nCells, a->d_ownerStart, a->d_losortStart,
-                                                                  a->d_losort, bs, a->d_bCellFaces, ssf_d, bssf_d,
-                                                                  V_d, out_d, divideByV, neiSign);
-    a->ctx->launches++;
-    KERNEL_CHECK();
-    return B200LDU_OK;
+    const BoundaryLists L = boundary_lists(a);
+    return with_nc(nComp, [&](auto nc) {
+        return launch(a->ctx, surface_integrate_kernel<nc>, a->nCells, 128, a->nCells, a->d_ownerStart, a->d_losortStart,
+                      a->d_losort, L.bStart, L.bFaces, ssf_d, bssf_d, V_d, out_d, divideByV, neiSign);
+    });
 }
 
 extern "C" int b200ldu_fv_gauss_grad(b200ldu_addr *a, int nComp, const double *Sf_d, const double *ssf_d,
@@ -79,19 +64,11 @@ extern "C" int b200ldu_fv_gauss_grad(b200ldu_addr *a, int nComp, const double *S
     if (!a || !Sf_d || !ssf_d || !V_d || !out_d || (nComp != 1 && nComp != 3)) return B200LDU_EINVAL;
     if (a->nBFaces && (!bSf_d || !bssf_d)) return B200LDU_EINVAL;
     CUDA_TRY(cudaSetDevice(a->ctx->device));
-    const int *bs = a->nBFaces ? a->d_bCellStart : nullptr;
-    dim3 g((a->nCells + 127) / 128), b(128);
-    if (nComp == 1)
-        gauss_grad_kernel<1><<<g, b, 0, a->ctx->stream>>>(a->nCells, a->d_ownerStart, a->d_losortStart,
-                                                           a->d_losort, bs, a->d_bCellFaces, Sf_d, ssf_d, bSf_d,
-                                                           bssf_d, V_d, out_d);
-    else
-        gauss_grad_kernel<3><<<g, b, 0, a->ctx->stream>>>(a->nCells, a->d_ownerStart, a->d_losortStart,
-                                                           a->d_losort, bs, a->d_bCellFaces, Sf_d, ssf_d, bSf_d,
-                                                           bssf_d, V_d, out_d);
-    a->ctx->launches++;
-    KERNEL_CHECK();
-    return B200LDU_OK;
+    const BoundaryLists L = boundary_lists(a);
+    return with_nc(nComp, [&](auto nc) {
+        return launch(a->ctx, gauss_grad_kernel<nc>, a->nCells, 128, a->nCells, a->d_ownerStart, a->d_losortStart,
+                      a->d_losort, L.bStart, L.bFaces, Sf_d, ssf_d, bSf_d, bssf_d, V_d, out_d);
+    });
 }
 
 // fused coefficient fills: one pass over the cells writes the diagonal as the negated
@@ -120,13 +97,9 @@ extern "C" int b200ldu_fv_laplacian_fill(b200ldu_addr *a, const double *deltaCoe
 {
     if (!a || !deltaCoeffs_d || !gammaMagSf_d || !upper_d || !diag_d) return B200LDU_EINVAL;
     CUDA_TRY(cudaSetDevice(a->ctx->device));
-    cudaStream_t st = a->ctx->stream;
-    if (a->nFaces) laplacian_upper_kernel<<<(a->nFaces + 255) / 256, 256, 0, st>>>(a->nFaces, deltaCoeffs_d, gammaMagSf_d, upper_d);
-    neg_sum_diag_kernel<<<(a->nCells + 127) / 128, 128, 0, st>>>(a->nCells, a->d_ownerStart, a->d_losortStart,
-                                                                  a->d_losort, upper_d, upper_d, diag_d);
-    a->ctx->launches += 2;
-    KERNEL_CHECK();
-    return B200LDU_OK;
+    TRY(launch(a->ctx, laplacian_upper_kernel, a->nFaces, 256, a->nFaces, deltaCoeffs_d, gammaMagSf_d, upper_d));
+    return launch(a->ctx, neg_sum_diag_kernel, a->nCells, 128, a->nCells, a->d_ownerStart, a->d_losortStart, a->d_losort,
+                  upper_d, upper_d, diag_d);
 }
 
 extern "C" int b200ldu_fv_convection_fill(b200ldu_addr *a, const double *weights_d, const double *phi_d,
@@ -134,13 +107,9 @@ extern "C" int b200ldu_fv_convection_fill(b200ldu_addr *a, const double *weights
 {
     if (!a || !weights_d || !phi_d || !lower_d || !upper_d || !diag_d) return B200LDU_EINVAL;
     CUDA_TRY(cudaSetDevice(a->ctx->device));
-    cudaStream_t st = a->ctx->stream;
-    if (a->nFaces) convection_faces_kernel<<<(a->nFaces + 255) / 256, 256, 0, st>>>(a->nFaces, weights_d, phi_d, lower_d, upper_d);
-    neg_sum_diag_kernel<<<(a->nCells + 127) / 128, 128, 0, st>>>(a->nCells, a->d_ownerStart, a->d_losortStart,
-                                                                  a->d_losort, upper_d, lower_d, diag_d);
-    a->ctx->launches += 2;
-    KERNEL_CHECK();
-    return B200LDU_OK;
+    TRY(launch(a->ctx, convection_faces_kernel, a->nFaces, 256, a->nFaces, weights_d, phi_d, lower_d, upper_d));
+    return launch(a->ctx, neg_sum_diag_kernel, a->nCells, 128, a->nCells, a->d_ownerStart, a->d_losortStart, a->d_losort,
+                  upper_d, lower_d, diag_d);
 }
 
 template <int NC>
@@ -162,15 +131,9 @@ extern "C" int b200ldu_fv_interpolate_linear(b200ldu_addr *a, int nComp, const d
 {
     if (!a || !w_d || !vf_d || !sf_d || (nComp != 1 && nComp != 3)) return B200LDU_EINVAL;
     CUDA_TRY(cudaSetDevice(a->ctx->device));
-    if (a->nFaces == 0) return B200LDU_OK;
-    dim3 g((a->nFaces + 255) / 256), b(256);
-    if (nComp == 1)
-        interpolate_linear_kernel<1><<<g, b, 0, a->ctx->stream>>>(a->nFaces, a->d_l, a->d_u, w_d, vf_d, sf_d);
-    else
-        interpolate_linear_kernel<3><<<g, b, 0, a->ctx->stream>>>(a->nFaces, a->d_l, a->d_u, w_d, vf_d, sf_d);
-    a->ctx->launches++;
-    KERNEL_CHECK();
-    return B200LDU_OK;
+    return with_nc(nComp, [&](auto nc) {
+        return launch(a->ctx, interpolate_linear_kernel<nc>, a->nFaces, 256, a->nFaces, a->d_l, a->d_u, w_d, vf_d, sf_d);
+    });
 }
 
 // x[cell] += sum of coeffs over the cell's boundary faces (ascending boundary face)
@@ -189,13 +152,10 @@ __global__ void add_boundary_kernel(int nCells, const int *__restrict__ bStart, 
 static int add_boundary(b200ldu_addr *a, const double *coeffs, double *x)
 {
     if (!a || !coeffs || !x) return B200LDU_EINVAL;
-    if (!a->nBFaces) return B200LDU_OK;
+    const BoundaryLists L = boundary_lists(a);
+    if (!L.bStart) return B200LDU_OK;
     CUDA_TRY(cudaSetDevice(a->ctx->device));
-    add_boundary_kernel<<<(a->nCells + 255) / 256, 256, 0, a->ctx->stream>>>(a->nCells, a->d_bCellStart,
-                                                                             a->d_bCellFaces, coeffs, x);
-    a->ctx->launches++;
-    KERNEL_CHECK();
-    return B200LDU_OK;
+    return launch(a->ctx, add_boundary_kernel, a->nCells, 256, a->nCells, L.bStart, L.bFaces, coeffs, x);
 }
 
 extern "C" int b200ldu_fv_add_boundary_diag(b200ldu_addr *a, const double *internalCoeffs_d, double *diag_d)
@@ -220,19 +180,11 @@ extern "C" int b200ldu_fv_grad_linear(b200ldu_addr *a, int nComp, const double *
     if (!a || !Sf_d || !w_d || !vf_d || !V_d || !out_d || (nComp != 1 && nComp != 3)) return B200LDU_EINVAL;
     if (a->nBFaces && (!bSf_d || !bvf_d)) return B200LDU_EINVAL;
     CUDA_TRY(cudaSetDevice(a->ctx->device));
-    const int *bs = a->nBFaces ? a->d_bCellStart : nullptr;
-    dim3 g((a->nCells + 127) / 128), b(128);
-    if (nComp == 1)
-        grad_linear_kernel<1><<<g, b, 0, a->ctx->stream>>>(a->nCells, a->d_ownerStart, a->d_u, a->d_losortStart,
-                                                            a->d_losort, a->d_l, bs, a->d_bCellFaces, Sf_d, w_d, vf_d,
-                                                            bSf_d, bvf_d, V_d, out_d);
-    else
-        grad_linear_kernel<3><<<g, b, 0, a->ctx->stream>>>(a->nCells, a->d_ownerStart, a->d_u, a->d_losortStart,
-                                                            a->d_losort, a->d_l, bs, a->d_bCellFaces, Sf_d, w_d, vf_d,
-                                                            bSf_d, bvf_d, V_d, out_d);
-    a->ctx->launches++;
-    KERNEL_CHECK();
-    return B200LDU_OK;
+    const BoundaryLists L = boundary_lists(a);
+    return with_nc(nComp, [&](auto nc) {
+        return launch(a->ctx, grad_linear_kernel<nc>, a->nCells, 128, a->nCells, a->d_ownerStart, a->d_u, a->d_losortStart,
+                      a->d_losort, a->d_l, L.bStart, L.bFaces, Sf_d, w_d, vf_d, bSf_d, bvf_d, V_d, out_d);
+    });
 }
 
 // phi = interpolate(U) & Sf per internal face (icoFoam.C:73-78 phiHbyA; face-parallel):
@@ -260,10 +212,5 @@ extern "C" int b200ldu_fv_flux_linear(b200ldu_addr *a, const double *Sf_d, const
 {
     if (!a || !Sf_d || !w_d || !U_d || !phi_d) return B200LDU_EINVAL;
     CUDA_TRY(cudaSetDevice(a->ctx->device));
-    if (a->nFaces == 0) return B200LDU_OK;
-    flux_linear_kernel<<<(a->nFaces + 255) / 256, 256, 0, a->ctx->stream>>>(a->nFaces, a->d_l, a->d_u, Sf_d, w_d, U_d,
-                                                                             phi_d);
-    a->ctx->launches++;
-    KERNEL_CHECK();
-    return B200LDU_OK;
+    return launch(a->ctx, flux_linear_kernel, a->nFaces, 256, a->nFaces, a->d_l, a->d_u, Sf_d, w_d, U_d, phi_d);
 }

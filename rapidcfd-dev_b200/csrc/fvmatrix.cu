@@ -25,35 +25,6 @@ using namespace fvmk;
 
 namespace
 {
-int coupled_lists(b200ldu_addr *a)
-{
-    if (a->d_cCellStart || a->nPatches == 0) return B200LDU_OK;
-    const int tot = a->patchStart.empty() ? 0 : a->patchStart[a->nPatches];
-    if (tot == 0) return B200LDU_OK;
-    std::vector<int> start((size_t)a->nCells + 1, 0), faces((size_t)tot);
-    for (int i = 0; i < tot; i++) start[a->faceCells[i] + 1]++;
-    for (int c = 0; c < a->nCells; c++) start[c + 1] += start[c];
-    std::vector<int> cur(start.begin(), start.end() - 1);
-    for (int i = 0; i < tot; i++) faces[cur[a->faceCells[i]]++] = i;
-    TRY(a->mem.upload(a->d_cCellStart, start));
-    TRY(a->mem.upload(a->d_cCellFaces, faces));
-    TRY(a->mem.upload(a->d_cFaceCells, a->faceCells));
-    a->nCFaces = tot;
-    return B200LDU_OK;
-}
-
-int lists(b200ldu_addr *a, BoundaryLists *L)
-{
-    TRY(coupled_lists(a));
-    L->bStart = a->nBFaces ? a->d_bCellStart : nullptr;
-    L->bFaces = a->d_bCellFaces;
-    L->cStart = a->nCFaces ? a->d_cCellStart : nullptr;
-    L->cFaces = a->d_cCellFaces;
-    return B200LDU_OK;
-}
-
-inline dim3 grid(int n, int b) { return dim3((unsigned)((n + b - 1) / b)); }
-
 bool bad_nc(int nc) { return nc != 1 && nc != 3; }
 
 int need_boundary(const b200ldu_addr *a, const void *ic, const char *what)
@@ -71,16 +42,14 @@ int need_boundary(const b200ldu_addr *a, const void *ic, const char *what)
 extern "C" int b200ldu_fv_patch_neighbour_field(b200ldu_addr *a, int nComp, const double *field_d, double *pnf_d)
 {
     if (!a || !field_d || bad_nc(nComp)) return B200LDU_EINVAL;
-    CUDA_TRY(cudaSetDevice(a->ctx->device));
-    TRY(coupled_lists(a));
-    if (a->nCFaces == 0) return B200LDU_OK;
+    const int nCFaces = a->L.nRecv;
+    if (nCFaces == 0) return B200LDU_OK;
     if (!pnf_d) return B200LDU_EINVAL;
+    CUDA_TRY(cudaSetDevice(a->ctx->device));
     double *send = nullptr;
-    TRY(a->mem.slot(ADDR_FVM_CMPT_PSI, send, (size_t)a->nCFaces * nComp));
-    fieldk::gather_kernel<<<grid(a->nCFaces * nComp, 256), 256, 0, a->ctx->stream>>>(a->nCFaces, nComp, a->d_cFaceCells,
-                                                                                      field_d, send);
-    a->ctx->launches++;
-    KERNEL_CHECK();
+    TRY(a->mem.slot(ADDR_FVM_CMPT_PSI, send, (size_t)nCFaces * nComp));
+    TRY(launch(a->ctx, fieldk::gather_kernel, (long long)nCFaces * nComp, 256, nCFaces, nComp, a->d_cFaceCells, field_d,
+               send));
     return comm_exchange_patch_field(a, nComp, send, pnf_d);
 }
 
@@ -91,13 +60,8 @@ extern "C" int b200ldu_fvm_add_boundary_diag(b200ldu_matrix *m, int nComp, int c
     b200ldu_addr *a = m->a;
     TRY(need_boundary(a, internalCoeffs_d, "fvm_add_boundary_diag"));
     CUDA_TRY(cudaSetDevice(a->ctx->device));
-    BoundaryLists L;
-    TRY(lists(a, &L));
-    boundary_diag_kernel<<<grid(a->nCells, 256), 256, 0, a->ctx->stream>>>(a->nCells, L, internalCoeffs_d, nComp, cmpt,
-                                                                           m->int_ext, diagIn_d, diagOut_d);
-    a->ctx->launches++;
-    KERNEL_CHECK();
-    return B200LDU_OK;
+    return launch(a->ctx, boundary_diag_kernel, a->nCells, 256, a->nCells, boundary_lists(a), internalCoeffs_d, nComp, cmpt,
+                  m->int_ext, diagIn_d, diagOut_d);
 }
 
 extern "C" int b200ldu_fvm_add_boundary_source(b200ldu_matrix *m, int nComp, const double *boundaryCoeffs_d,
@@ -107,17 +71,10 @@ extern "C" int b200ldu_fvm_add_boundary_source(b200ldu_matrix *m, int nComp, con
     b200ldu_addr *a = m->a;
     TRY(need_boundary(a, boundaryCoeffs_d, "fvm_add_boundary_source"));
     CUDA_TRY(cudaSetDevice(a->ctx->device));
-    BoundaryLists L;
-    TRY(lists(a, &L));
-    if (nComp == 1)
-        boundary_source_kernel<1><<<grid(a->nCells, 256), 256, 0, a->ctx->stream>>>(a->nCells, L, boundaryCoeffs_d,
-                                                                                    m->bou_ext, pnf_d, sourceIn_d, sourceOut_d);
-    else
-        boundary_source_kernel<3><<<grid(a->nCells, 256), 256, 0, a->ctx->stream>>>(a->nCells, L, boundaryCoeffs_d,
-                                                                                    m->bou_ext, pnf_d, sourceIn_d, sourceOut_d);
-    a->ctx->launches++;
-    KERNEL_CHECK();
-    return B200LDU_OK;
+    return with_nc(nComp, [&](auto nc) {
+        return launch(a->ctx, boundary_source_kernel<nc>, a->nCells, 256, a->nCells, boundary_lists(a), boundaryCoeffs_d,
+                      m->bou_ext, pnf_d, sourceIn_d, sourceOut_d);
+    });
 }
 
 extern "C" int b200ldu_fvm_A(b200ldu_matrix *m, int nComp, const double *internalCoeffs_d, const double *V_d,
@@ -127,13 +84,8 @@ extern "C" int b200ldu_fvm_A(b200ldu_matrix *m, int nComp, const double *interna
     b200ldu_addr *a = m->a;
     TRY(need_boundary(a, internalCoeffs_d, "fvm_A"));
     CUDA_TRY(cudaSetDevice(a->ctx->device));
-    BoundaryLists L;
-    TRY(lists(a, &L));
-    A_kernel<<<grid(a->nCells, 256), 256, 0, a->ctx->stream>>>(a->nCells, L, internalCoeffs_d, nComp, m->int_ext,
-                                                               m->diag_ext, V_d, A_d);
-    a->ctx->launches++;
-    KERNEL_CHECK();
-    return B200LDU_OK;
+    return launch(a->ctx, A_kernel, a->nCells, 256, a->nCells, boundary_lists(a), internalCoeffs_d, nComp, m->int_ext,
+                  m->diag_ext, V_d, A_d);
 }
 
 extern "C" int b200ldu_fvm_H(b200ldu_matrix *m, int nComp, const double *psi_d, const double *source_d,
@@ -142,24 +94,16 @@ extern "C" int b200ldu_fvm_H(b200ldu_matrix *m, int nComp, const double *psi_d, 
     if (!m || !psi_d || !source_d || !V_d || !H_d || bad_nc(nComp) || !m->diag_ext) return B200LDU_EINVAL;
     b200ldu_addr *a = m->a;
     TRY(need_boundary(a, boundaryCoeffs_d, "fvm_H"));
-    CUDA_TRY(cudaSetDevice(a->ctx->device));
-    BoundaryLists L;
-    TRY(lists(a, &L));
+    const BoundaryLists L = boundary_lists(a);
     if (L.cStart && !pnf_d) {
         b200_set_error("fvm_H: the coupled patches need their patchNeighbourField (fvMatrix.C:318-346)");
         return B200LDU_EINVAL;
     }
-    if (nComp == 1)
-        H_kernel<1><<<grid(a->nCells, 128), 128, 0, a->ctx->stream>>>(
-            a->nCells, a->d_ownerStart, a->d_u, a->d_losortStart, a->d_losort, a->d_l, m->upper_ext, m->lower_ext, L,
-            boundaryCoeffs_d, m->bou_ext, pnf_d, psi_d, source_d, V_d, H_d);
-    else
-        H_kernel<3><<<grid(a->nCells, 128), 128, 0, a->ctx->stream>>>(
-            a->nCells, a->d_ownerStart, a->d_u, a->d_losortStart, a->d_losort, a->d_l, m->upper_ext, m->lower_ext, L,
-            boundaryCoeffs_d, m->bou_ext, pnf_d, psi_d, source_d, V_d, H_d);
-    a->ctx->launches++;
-    KERNEL_CHECK();
-    return B200LDU_OK;
+    CUDA_TRY(cudaSetDevice(a->ctx->device));
+    return with_nc(nComp, [&](auto nc) {
+        return launch(a->ctx, H_kernel<nc>, a->nCells, 128, a->nCells, a->d_ownerStart, a->d_u, a->d_losortStart, a->d_losort,
+                      a->d_l, m->upper_ext, m->lower_ext, L, boundaryCoeffs_d, m->bou_ext, pnf_d, psi_d, source_d, V_d, H_d);
+    });
 }
 
 extern "C" int b200ldu_fvm_flux(b200ldu_matrix *m, int nComp, const double *psi_d, const double *internalCoeffs_d,
@@ -170,45 +114,21 @@ extern "C" int b200ldu_fvm_flux(b200ldu_matrix *m, int nComp, const double *psi_
     b200ldu_addr *a = m->a;
     if ((a->nFaces && !flux_d) || (a->nBFaces && (!boundaryFlux_d || !internalCoeffs_d || !boundaryCoeffs_d)))
         return B200LDU_EINVAL;
-    CUDA_TRY(cudaSetDevice(a->ctx->device));
-    BoundaryLists L;
-    TRY(lists(a, &L));
-    if (a->nCFaces && (!coupledFlux_d || !pnf_d)) {
+    const int nCFaces = a->L.nRecv;
+    if (nCFaces && (!coupledFlux_d || !pnf_d)) {
         b200_set_error("fvm_flux: the coupled patches need their patchNeighbourField and an output (fvMatrix.C:1636-1648)");
         return B200LDU_EINVAL;
     }
-    cudaStream_t st = a->ctx->stream;
-    if (a->nFaces) {
-        if (nComp == 1)
-            flux_internal_kernel<1><<<grid(a->nFaces, 256), 256, 0, st>>>(a->nFaces, a->d_l, a->d_u, m->upper_ext,
-                                                                          m->lower_ext, psi_d, flux_d);
-        else
-            flux_internal_kernel<3><<<grid(a->nFaces, 256), 256, 0, st>>>(a->nFaces, a->d_l, a->d_u, m->upper_ext,
-                                                                          m->lower_ext, psi_d, flux_d);
-        a->ctx->launches++;
-    }
-    if (a->nBFaces) {
-        if (nComp == 1)
-            flux_boundary_kernel<1><<<grid(a->nBFaces, 256), 256, 0, st>>>(a->nBFaces, a->d_bFaceCells, internalCoeffs_d,
-                                                                           1, boundaryCoeffs_d, 1, nullptr, psi_d,
-                                                                           boundaryFlux_d);
-        else
-            flux_boundary_kernel<3><<<grid(a->nBFaces, 256), 256, 0, st>>>(a->nBFaces, a->d_bFaceCells, internalCoeffs_d,
-                                                                           3, boundaryCoeffs_d, 3, nullptr, psi_d,
-                                                                           boundaryFlux_d);
-        a->ctx->launches++;
-    }
-    if (a->nCFaces) {
-        if (nComp == 1)
-            flux_boundary_kernel<1><<<grid(a->nCFaces, 256), 256, 0, st>>>(a->nCFaces, a->d_cFaceCells, m->int_ext, 1,
-                                                                           m->bou_ext, 1, pnf_d, psi_d, coupledFlux_d);
-        else
-            flux_boundary_kernel<3><<<grid(a->nCFaces, 256), 256, 0, st>>>(a->nCFaces, a->d_cFaceCells, m->int_ext, 1,
-                                                                           m->bou_ext, 1, pnf_d, psi_d, coupledFlux_d);
-        a->ctx->launches++;
-    }
-    KERNEL_CHECK();
-    return B200LDU_OK;
+    CUDA_TRY(cudaSetDevice(a->ctx->device));
+    b200ldu_ctx *ctx = a->ctx;
+    return with_nc(nComp, [&](auto nc) {
+        TRY(launch(ctx, flux_internal_kernel<nc>, a->nFaces, 256, a->nFaces, a->d_l, a->d_u, m->upper_ext, m->lower_ext, psi_d,
+                   flux_d));
+        TRY(launch(ctx, flux_boundary_kernel<nc>, a->nBFaces, 256, a->nBFaces, a->d_bFaceCells, internalCoeffs_d, int(nc),
+                   boundaryCoeffs_d, int(nc), nullptr, psi_d, boundaryFlux_d));
+        return launch(ctx, flux_boundary_kernel<nc>, nCFaces, 256, nCFaces, a->d_cFaceCells, m->int_ext, 1, m->bou_ext, 1,
+                      pnf_d, psi_d, coupledFlux_d);
+    });
 }
 
 extern "C" int b200ldu_fvm_residual(b200ldu_matrix *m, const double *psi_d, const double *source_d,
@@ -219,19 +139,16 @@ extern "C" int b200ldu_fvm_residual(b200ldu_matrix *m, const double *psi_d, cons
     b200ldu_addr *a = m->a;
     TRY(need_boundary(a, internalCoeffs_d, "fvm_residual"));
     TRY(need_boundary(a, boundaryCoeffs_d, "fvm_residual"));
-    CUDA_TRY(cudaSetDevice(a->ctx->device));
-    BoundaryLists L;
-    TRY(lists(a, &L));
+    const BoundaryLists L = boundary_lists(a);
     if (L.cStart && !pnf_d) {
         b200_set_error("fvm_residual: the coupled patches need their patchNeighbourField (addBoundarySource)");
         return B200LDU_EINVAL;
     }
+    CUDA_TRY(cudaSetDevice(a->ctx->device));
     double *tmp = nullptr;
     TRY(a->mem.slot(ADDR_FVM_DIAG, tmp, (size_t)a->nCells));
-    residual_source_kernel<<<grid(a->nCells, 256), 256, 0, a->ctx->stream>>>(a->nCells, L, internalCoeffs_d, m->int_ext,
-                                                                             psi_d, source_d, tmp);
-    a->ctx->launches++;
-    KERNEL_CHECK();
+    TRY(launch(a->ctx, residual_source_kernel, a->nCells, 256, a->nCells, L, internalCoeffs_d, m->int_ext, psi_d, source_d,
+               tmp));
     TRY(b200ldu_residual(m, psi_d, tmp, residual_d)); // lduMatrix::residual incl. the interface update
     return b200ldu_fvm_add_boundary_source(m, 1, boundaryCoeffs_d, pnf_d, residual_d, residual_d);
 }
@@ -244,19 +161,11 @@ extern "C" int b200ldu_fvm_relax(b200ldu_matrix *m, int nComp, double alpha, con
     b200ldu_addr *a = m->a;
     TRY(need_boundary(a, internalCoeffs_d, "fvm_relax"));
     CUDA_TRY(cudaSetDevice(a->ctx->device));
-    BoundaryLists L;
-    TRY(lists(a, &L));
-    if (nComp == 1)
-        relax_kernel<1><<<grid(a->nCells, 128), 128, 0, a->ctx->stream>>>(
-            a->nCells, a->d_ownerStart, a->d_losortStart, a->d_losort, m->upper_ext, m->lower_ext, L, internalCoeffs_d,
-            m->int_ext, m->bou_ext, alpha, psi_d, diag_d, source_d);
-    else
-        relax_kernel<3><<<grid(a->nCells, 128), 128, 0, a->ctx->stream>>>(
-            a->nCells, a->d_ownerStart, a->d_losortStart, a->d_losort, m->upper_ext, m->lower_ext, L, internalCoeffs_d,
-            m->int_ext, m->bou_ext, alpha, psi_d, diag_d, source_d);
-    a->ctx->launches++;
-    KERNEL_CHECK();
-    return B200LDU_OK;
+    return with_nc(nComp, [&](auto nc) {
+        return launch(a->ctx, relax_kernel<nc>, a->nCells, 128, a->nCells, a->d_ownerStart, a->d_losortStart, a->d_losort,
+                      m->upper_ext, m->lower_ext, boundary_lists(a), internalCoeffs_d, m->int_ext, m->bou_ext, alpha, psi_d,
+                      diag_d, source_d);
+    });
 }
 
 extern "C" int b200ldu_fvm_set_reference(b200ldu_matrix *m, int celli, int nComp, const double *value_h,
@@ -266,11 +175,8 @@ extern "C" int b200ldu_fvm_set_reference(b200ldu_matrix *m, int celli, int nComp
     if (celli < 0) return B200LDU_OK; // the reference cell lives on another rank (fvMatrix.C:972)
     b200ldu_addr *a = m->a;
     CUDA_TRY(cudaSetDevice(a->ctx->device));
-    set_reference_kernel<<<1, 1, 0, a->ctx->stream>>>(celli, nComp, value_h[0], nComp > 1 ? value_h[1] : 0.0,
-                                                      nComp > 2 ? value_h[2] : 0.0, diag_d, source_d);
-    a->ctx->launches++;
-    KERNEL_CHECK();
-    return B200LDU_OK;
+    return launch(a->ctx, set_reference_kernel, 1, 1, celli, nComp, value_h[0], nComp > 1 ? value_h[1] : 0.0,
+                  nComp > 2 ? value_h[2] : 0.0, diag_d, source_d);
 }
 
 // solveSegregated: fold the boundary into diagonal and source, solve, put the diagonal back.
@@ -285,50 +191,44 @@ extern "C" int b200ldu_fvm_solve(b200ldu_matrix *m, int nComp, const char *solve
     b200ldu_addr *a = m->a;
     TRY(need_boundary(a, internalCoeffs_d, "fvm_solve"));
     TRY(need_boundary(a, boundaryCoeffs_d, "fvm_solve"));
-    CUDA_TRY(cudaSetDevice(a->ctx->device));
-    BoundaryLists L;
-    TRY(lists(a, &L));
+    const BoundaryLists L = boundary_lists(a);
     if (nComp > 1 && L.cStart && !pnf_d) {
         b200_set_error("fvm_solve: the component loop needs the patchNeighbourField of the coupled patches");
         return B200LDU_EINVAL;
     }
+    CUDA_TRY(cudaSetDevice(a->ctx->device));
+    b200ldu_ctx *ctx = a->ctx;
     const int n = a->nCells;
-    cudaStream_t st = a->ctx->stream;
     // the caller's coefficient arrays: the matrix is re-pointed at the folded diagonal for the solve
     const double *diag0 = m->diag_ext;
     const double *bou = m->bou_ext, *intc = m->int_ext;
     double *dK = nullptr, *total = nullptr, *sK = nullptr, *pK = nullptr;
     TRY(a->mem.slot(ADDR_FVM_DIAG, dK, (size_t)n));
     TRY(a->mem.slot(ADDR_FVM_SOURCE, total, (size_t)n * nComp));
+    if (nComp > 1) {
+        TRY(a->mem.slot(ADDR_FVM_CMPT_SOURCE, sK, (size_t)n));
+        TRY(a->mem.slot(ADDR_FVM_CMPT_PSI, pK, (size_t)n));
+    }
+    // a scalar takes the coupled boundary source through the solve's interface update, a vector once here
+    if (nComp == 1) TRY(launch(ctx, boundary_diag_kernel, n, 256, n, L, internalCoeffs_d, 1, 0, intc, diag0, dK));
+    TRY(with_nc(nComp, [&](auto nc) {
+        return launch(ctx, boundary_source_kernel<nc>, n, 256, n, L, boundaryCoeffs_d, bou, nc == 1 ? nullptr : pnf_d,
+                      source_d, total);
+    }));
     int rc = B200LDU_OK;
     if (nComp == 1) {
-        boundary_diag_kernel<<<grid(n, 256), 256, 0, st>>>(n, L, internalCoeffs_d, 1, 0, intc, diag0, dK);
-        boundary_source_kernel<1><<<grid(n, 256), 256, 0, st>>>(n, L, boundaryCoeffs_d, bou, nullptr, source_d, total);
-        a->ctx->launches += 2;
-        KERNEL_CHECK();
         rc = matrix_set_diag(m, dK); // the off-diagonal streams are unchanged
         if (rc == B200LDU_OK) rc = b200ldu_solve(m, solver, precondOrSmoother, controls, gamg, psi_d, total, &perf[0], nullptr, 0);
     } else {
-        TRY(a->mem.slot(ADDR_FVM_CMPT_SOURCE, sK, (size_t)n));
-        TRY(a->mem.slot(ADDR_FVM_CMPT_PSI, pK, (size_t)n));
-        boundary_source_kernel<3><<<grid(n, 256), 256, 0, st>>>(n, L, boundaryCoeffs_d, bou, pnf_d, source_d, total);
-        a->ctx->launches++;
-        KERNEL_CHECK();
         BoundaryLists none = L;
         none.cStart = nullptr;
         for (int k = 0; k < nComp && rc == B200LDU_OK; k++) {
-            boundary_diag_kernel<<<grid(n, 256), 256, 0, st>>>(n, L, internalCoeffs_d, nComp, k, intc, diag0, dK);
-            component_kernel<<<grid(n, 256), 256, 0, st>>>(n, nComp, k, L, bou, pnf_d, total, sK);
-            component_kernel<<<grid(n, 256), 256, 0, st>>>(n, nComp, k, none, nullptr, nullptr, psi_d, pK);
-            a->ctx->launches += 3;
-            KERNEL_CHECK();
+            TRY(launch(ctx, boundary_diag_kernel, n, 256, n, L, internalCoeffs_d, nComp, k, intc, diag0, dK));
+            TRY(launch(ctx, component_kernel, n, 256, n, nComp, k, L, bou, pnf_d, total, sK));
+            TRY(launch(ctx, component_kernel, n, 256, n, nComp, k, none, nullptr, nullptr, psi_d, pK));
             rc = matrix_set_diag(m, dK);
             if (rc == B200LDU_OK) rc = b200ldu_solve(m, solver, precondOrSmoother, controls, gamg, pK, sK, &perf[k], nullptr, 0);
-            if (rc == B200LDU_OK) {
-                set_component_kernel<<<grid(n, 256), 256, 0, st>>>(n, nComp, k, pK, psi_d);
-                a->ctx->launches++;
-                KERNEL_CHECK();
-            }
+            if (rc == B200LDU_OK) TRY(launch(ctx, set_component_kernel, n, 256, n, nComp, k, pK, psi_d));
         }
     }
     const int rc2 = matrix_set_diag(m, diag0); // diag() = saveDiag

@@ -5,14 +5,12 @@
 #define B200LDU_FVMATRIX_KERNELS_CUH
 #include <cstddef>
 
+#include "boundary_lists.cuh"
+
 namespace fvmk
 {
 namespace // internal linkage: the headers are included by more than one translation unit
 {
-struct BoundaryLists { // per-cell CSR over the non-coupled boundary faces and over the coupled patch faces
-    const int *bStart, *bFaces, *cStart, *cFaces;
-};
-
 __device__ __forceinline__ double cmpt_av(const double *v, int nc) // VectorSpaceI.H:428-447: ((x + y) + z)/3
 {
     if (nc == 1) return v[0];

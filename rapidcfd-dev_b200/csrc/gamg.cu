@@ -203,18 +203,6 @@ static void coarse_addressing(const std::vector<int> &lo, const std::vector<int>
         }
 }
 
-static void csr_from_map(const std::vector<int> &map, int nTargets, std::vector<int> &start, std::vector<int> &items)
-{
-    start.assign((size_t)nTargets + 1, 0);
-    for (int v : map)
-        if (v >= 0) start[v + 1]++;
-    for (int t = 0; t < nTargets; t++) start[t + 1] += start[t];
-    items.resize(std::max(start[nTargets], 1));
-    std::vector<int> cur(start.begin(), start.end() - 1);
-    for (int i = 0; i < (int)map.size(); i++)
-        if (map[i] >= 0) items[cur[map[i]]++] = i;
-}
-
 // continueAgglomerating (GAMGAgglomeration.C:72-84): and-reduced over the ranks (ctx null: one rank)
 static int continue_vote(b200ldu_ctx *ctx, bool mine, bool &cont)
 {
@@ -692,15 +680,6 @@ __global__ void dense_apply_kernel(int n, const double *__restrict__ inv, const 
 // ---------------------------------------------------------------------------
 namespace {
 
-// kernel(n, args...) with one thread per item, 256 per CTA, on the solve's stream; n <= 0 launches nothing
-template <class... P, class... A>
-void launch1d(Solve &S, void (*kernel)(int, P...), int n, A... args)
-{
-    if (n <= 0) return;
-    kernel<<<(n + 255) / 256, 256, 0, S.ctx->stream>>>(n, args...);
-    S.ctx->launches++;
-}
-
 int smooth_in_place(Solve &S, b200ldu_matrix *m, double omega, double *&x, double *&spare, const double *b,
                     int nSweeps, const int *stop)
 {
@@ -746,11 +725,12 @@ static int gamg_build_matrices(Solve &S, b200ldu_gamg *g)
     }
     for (int k = 0; k < g->nLevels; k++) {
         GamgLevel &L = g->lev[k];
-        launch1d(S, agg_diag_kernel, L.nCoarse, L.d_cellChildStart, L.d_cellChild, L.d_diagFaceStart, L.d_diagFace, fd,
-                 fu, fl, L.d_diag);
-        launch1d(S, agg_faces_kernel, L.nCoarseFaces, L.d_faceChildStart, L.d_faceChild, fu, fl, L.d_upper, L.d_lower);
-        launch1d(S, agg_patch_kernel, L.nCoarsePF, L.d_pfChildStart, L.d_pfChild, fb, fi, L.d_bou, L.d_int);
-        KERNEL_CHECK();
+        TRY(launch(S.ctx, agg_diag_kernel, L.nCoarse, 256, L.nCoarse, L.d_cellChildStart, L.d_cellChild,
+                   L.d_diagFaceStart, L.d_diagFace, fd, fu, fl, L.d_diag));
+        TRY(launch(S.ctx, agg_faces_kernel, L.nCoarseFaces, 256, L.nCoarseFaces, L.d_faceChildStart, L.d_faceChild, fu,
+                   fl, L.d_upper, L.d_lower));
+        TRY(launch(S.ctx, agg_patch_kernel, L.nCoarsePF, 256, L.nCoarsePF, L.d_pfChildStart, L.d_pfChild, fb, fi,
+                   L.d_bou, L.d_int));
         // identical boundary/internal interface coefficients on the finest level stay identical
         const double *cInt = (fm->bou_ext == fm->int_ext) ? L.d_bou : L.d_int;
         TRY(b200ldu_matrix_set(L.mat, L.d_diag, L.d_upper, fl ? L.d_lower : nullptr, L.nCoarsePF > 0 ? L.d_bou : nullptr,
@@ -885,7 +865,8 @@ static int gamg_cycle(Solve &S, b200ldu_gamg *g, int scaleCorrection, double *co
     // ---- Vcycle (GAMGSolverSolve.C:181-474) ----
     {
         GamgLevel &L0 = g->lev[0];
-        launch1d(S, restrict_kernel, L0.nCoarse, L0.d_childStart, L0.d_child, finestRes, L0.src, stop);
+        TRY(launch(S.ctx, restrict_kernel, L0.nCoarse, 256, L0.nCoarse, L0.d_childStart, L0.d_child, finestRes, L0.src,
+                   stop));
     }
     for (int k = 0; k < coarsest; k++) {
         GamgLevel &L = g->lev[k], &Ln = g->lev[k + 1];
@@ -901,7 +882,8 @@ static int gamg_cycle(Solve &S, b200ldu_gamg *g, int scaleCorrection, double *co
                 V2(src)[i] = make_double2(__dsub_rn(s2.x, a2.x), __dsub_rn(s2.y, a2.y));
             }));
         }
-        launch1d(S, restrict_kernel, Ln.nCoarse, Ln.d_childStart, Ln.d_child, L.src, Ln.src, stop);
+        TRY(launch(S.ctx, restrict_kernel, Ln.nCoarse, 256, Ln.nCoarse, Ln.d_childStart, Ln.d_child, L.src, Ln.src,
+                   stop));
     }
     { // solveCoarsestLevel :552-619
         GamgLevel &L = g->lev[coarsest];
@@ -968,7 +950,7 @@ static int gamg_cycle(Solve &S, b200ldu_gamg *g, int scaleCorrection, double *co
         int nPadL = L.addr->L.nPad;
         if (c.nPreSweeps)
             CUDA_TRY(cudaMemcpyAsync(L.pre, L.corr, sizeof(double) * (size_t)L.addr->vecLen, cudaMemcpyDeviceToDevice, st));
-        launch1d(S, prolong_kernel, nPadL, Ln.d_pmap, Ln.corr, L.corr, stop);
+        TRY(launch(S.ctx, prolong_kernel, nPadL, 256, nPadL, Ln.d_pmap, Ln.corr, L.corr, stop));
         if (c.interpolateCorrection) {
             TRY(mat_interpolate(L.mat, L.corr, L.tmp, stop));
             std::swap(L.corr, L.tmp);
@@ -987,8 +969,7 @@ static int gamg_cycle(Solve &S, b200ldu_gamg *g, int scaleCorrection, double *co
     }
     {
         GamgLevel &L0 = g->lev[0];
-        launch1d(S, prolong_kernel, fm->a->L.nPad, L0.d_pmap, L0.corr, finestCorr, stop);
-        KERNEL_CHECK();
+        TRY(launch(S.ctx, prolong_kernel, fm->a->L.nPad, 256, fm->a->L.nPad, L0.d_pmap, L0.corr, finestCorr, stop));
     }
     double *psi = psiBuf[finestSweeps & 1], *spare = psiBuf[(finestSweeps + 1) & 1];
     if (c.interpolateCorrection) {

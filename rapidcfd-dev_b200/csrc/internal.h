@@ -5,10 +5,13 @@
 #include <stdio.h>
 #include <string.h>
 
+#include <algorithm>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/b200ldu.h"
+#include "boundary_lists.cuh"
 
 // ---------------------------------------------------------------------------
 // error handling: nothing throws across the ABI
@@ -298,8 +301,7 @@ struct b200ldu_addr {
     int nBFaces = 0;
     int *d_bFaceCells = nullptr;
     int *d_bCellStart = nullptr, *d_bCellFaces = nullptr;
-    // fvMatrix glue (fvmatrix.cu): per-cell lists over the coupled patch faces, built at first use
-    int nCFaces = 0;
+    // coupled patch faces (L.nRecv of them, patch order): per-cell lists and the face cells, uploaded when there are any
     int *d_cCellStart = nullptr, *d_cCellFaces = nullptr, *d_cFaceCells = nullptr;
     // host-only structural self-check (b200ldu_layout_debug_*): no GPU, no compute
     bool hostOnly = false;
@@ -353,4 +355,44 @@ inline double *banded_vec(const b200ldu_addr *a, DeviceMem &mem, int k)
 {
     double *d = nullptr;
     return mem.slot(k, d, (size_t)a->vecLen, true) == B200LDU_OK ? d : nullptr;
+}
+
+// kernel<<<ceil(nItems / block), block>>>(args...) on ctx's stream, counted in ctx->launches; nItems <= 0 launches
+// nothing
+template <class... P, class... A>
+int launch(b200ldu_ctx *ctx, void (*kernel)(P...), long long nItems, int block, A... args)
+{
+    if (nItems <= 0) return B200LDU_OK;
+    kernel<<<(unsigned)((nItems + block - 1) / block), block, 0, ctx->stream>>>(args...);
+    ctx->launches++;
+    KERNEL_CHECK();
+    return B200LDU_OK;
+}
+
+// f(std::integral_constant<int, nComp>()) for a component count of 1 or 3 (the caller checks it)
+template <class F>
+int with_nc(int nComp, F f)
+{
+    return nComp == 1 ? f(std::integral_constant<int, 1>()) : f(std::integral_constant<int, 3>());
+}
+
+// stable counting sort: items of target t = the indices i with map[i] == t, ascending, at [start[t], start[t+1]);
+// negative map entries belong to no target
+inline void csr_from_map(const std::vector<int> &map, int nTargets, std::vector<int> &start, std::vector<int> &items)
+{
+    start.assign((size_t)nTargets + 1, 0);
+    for (int v : map)
+        if (v >= 0) start[v + 1]++;
+    for (int t = 0; t < nTargets; t++) start[t + 1] += start[t];
+    items.resize(std::max(start[nTargets], 1));
+    std::vector<int> cur(start.begin(), start.end() - 1);
+    for (int i = 0; i < (int)map.size(); i++)
+        if (map[i] >= 0) items[cur[map[i]]++] = i;
+}
+
+// the boundary lists of a as the finite-volume kernels take them; a list with no faces has a null start
+static inline fvmk::BoundaryLists boundary_lists(const b200ldu_addr *a)
+{
+    return {a->nBFaces ? a->d_bCellStart : nullptr, a->d_bCellFaces, a->L.nRecv ? a->d_cCellStart : nullptr,
+            a->d_cCellFaces};
 }

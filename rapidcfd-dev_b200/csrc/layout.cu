@@ -38,20 +38,8 @@ struct Graph {
     std::vector<int> pfStart, pfItem; // cell -> coupled-patch faces, in (patch, patch face) order
 };
 
-// cell -> faces it owns is contiguous (faces sorted by owner); cell -> faces where it
-// is neighbour needs the stable counting sort the reference calls losort.
-void build_losort(int nCells, const std::vector<int> &u, std::vector<int> &losortStart,
-                  std::vector<int> &losort)
-{
-    int nF = (int)u.size();
-    losortStart.assign((size_t)nCells + 1, 0);
-    for (int f = 0; f < nF; f++) losortStart[u[f] + 1]++;
-    for (int c = 0; c < nCells; c++) losortStart[c + 1] += losortStart[c];
-    losort.resize(nF);
-    std::vector<int> cur(losortStart.begin(), losortStart.end() - 1);
-    for (int f = 0; f < nF; f++) losort[cur[u[f]]++] = f;
-}
-
+// cell -> faces it owns is contiguous (faces sorted by owner); cell -> faces where it is neighbour is the stable
+// counting sort the reference calls losort (csr_from_map of the neighbours)
 void build_owner_start(int nCells, const std::vector<int> &l, std::vector<int> &ownerStart)
 {
     ownerStart.assign((size_t)nCells + 1, 0);
@@ -172,7 +160,7 @@ int build_csr(Graph &g)
         }
     }
     build_owner_start(g.nCells, g.l, g.ownerStart);
-    build_losort(g.nCells, g.u, g.losortStart, g.losort);
+    csr_from_map(g.u, g.nCells, g.losortStart, g.losort);
     return B200LDU_OK;
 }
 
@@ -256,16 +244,7 @@ std::vector<int> renumber(const Graph &g, const double *centres)
     return order;
 }
 
-// ---- 3. cell -> coupled-patch faces -------------------------------------------
-void build_patch_faces(const std::vector<int> &faceCells, Graph &g)
-{
-    g.pfStart.assign((size_t)g.nCells + 1, 0);
-    g.pfItem.resize(g.nRecv);
-    for (int i = 0; i < g.nRecv; i++) g.pfStart[faceCells[i] + 1]++;
-    for (int c = 0; c < g.nCells; c++) g.pfStart[c + 1] += g.pfStart[c];
-    std::vector<int> cur(g.pfStart.begin(), g.pfStart.end() - 1);
-    for (int i = 0; i < g.nRecv; i++) g.pfItem[cur[faceCells[i]]++] = i;
-}
+// ---- 3. cell -> coupled-patch faces: csr_from_map of the face cells (layout_build) ----
 
 // ---- 4. plan for one band size --------------------------------------------------
 // Everything but the two streams' entries: slice widths and offsets of both streams, the face stream's list bounds,
@@ -639,6 +618,11 @@ int layout_upload(b200ldu_addr *a, const Graph &g, const LayoutHost &H)
     TRY(mem.upload(a->d_ownerStart, g.ownerStart));
     TRY(mem.upload(a->d_losort, g.losort));
     TRY(mem.upload(a->d_losortStart, g.losortStart));
+    if (H.nRecv) {
+        TRY(mem.upload(a->d_cCellStart, g.pfStart));
+        TRY(mem.upload(a->d_cCellFaces, g.pfItem));
+        TRY(mem.upload(a->d_cFaceCells, a->faceCells));
+    }
     if (H.hasFs) {
         TRY(mem.upload(L.fsSlice, H.fsSlice));
         TRY(mem.upload(L.fsTpl, H.fsTpl));
@@ -675,7 +659,7 @@ int layout_build(b200ldu_addr *a, const double *centres)
     const std::vector<int> order = renumber(g, centres);
     a->perm_h.assign(g.nCells, 0);
     for (int r = 0; r < g.nCells; r++) a->perm_h[order[r]] = r;
-    build_patch_faces(a->faceCells, g);
+    csr_from_map(a->faceCells, g.nCells, g.pfStart, g.pfItem);
 
     int packCtas = 0;
     for (int p = 0; p < a->nPatches; p++)

@@ -248,19 +248,13 @@ __global__ void from_banded_kernel(int nCells, const int *__restrict__ iperm,
 
 int to_banded(b200ldu_addr *a, const double *x, double *xb)
 {
-    to_banded_kernel<<<(a->L.nPad + 255) / 256, 256, 0, a->ctx->stream>>>(a->L.nPad, a->L.iperm, x, xb);
-    a->ctx->launches++;
-    KERNEL_CHECK();
-    return B200LDU_OK;
+    return launch(a->ctx, to_banded_kernel, a->L.nPad, 256, a->L.nPad, a->L.iperm, x, xb);
 }
 
 int from_banded(b200ldu_addr *a, const double *xb, double *x)
 {
     // rows [0, nCells) are the real rows (padding sits at the end)
-    from_banded_kernel<<<(a->nCells + 255) / 256, 256, 0, a->ctx->stream>>>(a->nCells, a->L.iperm, xb, x);
-    a->ctx->launches++;
-    KERNEL_CHECK();
-    return B200LDU_OK;
+    return launch(a->ctx, from_banded_kernel, a->nCells, 256, a->nCells, a->L.iperm, xb, x);
 }
 
 extern "C" int b200ldu_to_banded(b200ldu_addr *a, const double *x_d, double *xb_d)
@@ -374,10 +368,7 @@ static int own_copy(b200ldu_matrix *m, int k, const double *src, size_t n, const
 int matrix_set_diag(b200ldu_matrix *m, const double *diag_d)
 {
     b200ldu_addr *a = m->a;
-    fill_diag_kernel<<<(unsigned)((a->vecLen + 255) / 256), 256, 0, a->ctx->stream>>>(a->vecLen, a->L.nPad, a->L.iperm,
-                                                                                      diag_d, m->d_diag, m->d_rD);
-    a->ctx->launches++;
-    KERNEL_CHECK();
+    TRY(launch(a->ctx, fill_diag_kernel, a->vecLen, 256, a->vecLen, a->L.nPad, a->L.iperm, diag_d, m->d_diag, m->d_rD));
     m->diag_ext = diag_d;
     return B200LDU_OK;
 }
@@ -395,7 +386,6 @@ extern "C" int b200ldu_matrix_set(b200ldu_matrix *m, const double *diag_d, const
         return B200LDU_EINVAL;
     }
     CUDA_TRY(cudaSetDevice(a->ctx->device));
-    cudaStream_t st = a->ctx->stream;
     m->symmetric = (lower_d == nullptr);
     const bool sameIfc = (bou_d == int_d);
     // The matrix keeps its own caller-order copies (the reference's lduMatrix owns diag/upper/lower,
@@ -421,10 +411,7 @@ extern "C" int b200ldu_matrix_set(b200ldu_matrix *m, const double *diag_d, const
         m->d_val = m->d_valT = nullptr;
         const long long nf = a->fsOwn + a->fsList;
         TRY(m->mem.slot(MAT_FVAL, m->d_fval, (size_t)nf));
-        if (nf > 0) {
-            fill_val_kernel<<<(unsigned)((nf + 255) / 256), 256, 0, st>>>(nf, a->d_fsCode, up, lo, bo, m->d_fval, 0);
-            a->ctx->launches++;
-        }
+        TRY(launch(a->ctx, fill_val_kernel, nf, 256, nf, a->d_fsCode, up, lo, bo, m->d_fval, 0));
     } else {
         m->mem.release(MAT_FVAL);
         m->d_fval = nullptr;
@@ -435,17 +422,9 @@ extern "C" int b200ldu_matrix_set(b200ldu_matrix *m, const double *diag_d, const
             m->mem.release(MAT_VALT);
             m->d_valT = m->d_val; // A^T == A
         }
-        if (ne > 0) {
-            unsigned g = (unsigned)((ne + 255) / 256);
-            fill_val_kernel<<<g, 256, 0, st>>>(ne, a->d_code, up, lo, bo, m->d_val, 0);
-            a->ctx->launches++;
-            if (needT) {
-                fill_val_kernel<<<g, 256, 0, st>>>(ne, a->d_code, up, lo, in, m->d_valT, 1);
-                a->ctx->launches++;
-            }
-        }
+        TRY(launch(a->ctx, fill_val_kernel, ne, 256, ne, a->d_code, up, lo, bo, m->d_val, 0));
+        if (needT) TRY(launch(a->ctx, fill_val_kernel, ne, 256, ne, a->d_code, up, lo, in, m->d_valT, 1));
     }
-    KERNEL_CHECK();
     m->haveT = needT;
     m->upper_ext = up;
     m->bou_ext = bo;
@@ -672,12 +651,8 @@ extern "C" int b200ldu_faceH(b200ldu_matrix *m, const double *psi_d, double *fac
         b200_set_error("faceH: the matrix does not have any off-diagonal coefficients");
         return B200LDU_EINVAL;
     }
-    if (a->nFaces == 0) return B200LDU_OK;
-    faceH_kernel<<<(a->nFaces + 255) / 256, 256, 0, a->ctx->stream>>>(a->nFaces, a->d_l, a->d_u, m->upper_ext,
-                                                                        m->lower_ext, psi_d, faceHpsi_d);
-    a->ctx->launches++;
-    KERNEL_CHECK();
-    return B200LDU_OK;
+    return launch(a->ctx, faceH_kernel, a->nFaces, 256, a->nFaces, a->d_l, a->d_u, m->upper_ext, m->lower_ext, psi_d,
+                  faceHpsi_d);
 }
 
 int precond_kind(const char *name, char *printed)

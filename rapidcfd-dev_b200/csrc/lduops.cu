@@ -52,11 +52,7 @@ __global__ void scale_kernel(long long n, const int *__restrict__ idx, const dou
 
 int axpy(b200ldu_ctx *ctx, long long n, int sub, int assign, const double *x, double *y)
 {
-    if (n <= 0) return B200LDU_OK;
-    axpy_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(n, sub, assign, x, y);
-    ctx->launches++;
-    KERNEL_CHECK();
-    return B200LDU_OK;
+    return launch(ctx, axpy_kernel, n, 256, n, sub, assign, x, y);
 }
 
 } // namespace
@@ -66,11 +62,8 @@ extern "C" int b200ldu_ldu_row_sum(b200ldu_addr *a, int mode, const double *uppe
 {
     if (!a || !inout_d || mode < 0 || mode > 2 || (a->nFaces && !upper_d)) return B200LDU_EINVAL;
     CUDA_TRY(cudaSetDevice(a->ctx->device));
-    row_sum_kernel<<<(a->nCells + 127) / 128, 128, 0, a->ctx->stream>>>(a->nCells, mode, a->d_ownerStart, a->d_losortStart,
-                                                                        a->d_losort, upper_d, lower_d ? lower_d : upper_d, inout_d);
-    a->ctx->launches++;
-    KERNEL_CHECK();
-    return B200LDU_OK;
+    return launch(a->ctx, row_sum_kernel, a->nCells, 128, a->nCells, mode, a->d_ownerStart, a->d_losortStart, a->d_losort,
+                  upper_d, lower_d ? lower_d : upper_d, inout_d);
 }
 
 // A (+|-)= B with the reference's rules for the kinds of the two matrices (lduMatrixOperations.C:235-397).
@@ -131,10 +124,8 @@ extern "C" int b200ldu_ldu_scale(b200ldu_addr *a, const double *sf_d, double s, 
     b200ldu_ctx *ctx = a->ctx;
     CUDA_TRY(cudaSetDevice(ctx->device));
     const long long n = a->nCells, nF = a->nFaces;
-    if (hasA[0] && diagA_d && n) scale_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(n, nullptr, sf_d, s, diagA_d);
-    if (hasA[1] && upperA_d && nF) scale_kernel<<<(unsigned)((nF + 255) / 256), 256, 0, ctx->stream>>>(nF, a->d_l, sf_d, s, upperA_d);
-    if (hasA[2] && lowerA_d && nF) scale_kernel<<<(unsigned)((nF + 255) / 256), 256, 0, ctx->stream>>>(nF, a->d_u, sf_d, s, lowerA_d);
-    ctx->launches += 3;
-    KERNEL_CHECK();
+    if (hasA[0] && diagA_d) TRY(launch(ctx, scale_kernel, n, 256, n, nullptr, sf_d, s, diagA_d));
+    if (hasA[1] && upperA_d) TRY(launch(ctx, scale_kernel, nF, 256, nF, a->d_l, sf_d, s, upperA_d));
+    if (hasA[2] && lowerA_d) TRY(launch(ctx, scale_kernel, nF, 256, nF, a->d_u, sf_d, s, lowerA_d));
     return B200LDU_OK;
 }

@@ -29,36 +29,28 @@ static int mules_limiter_impl(int corr, double extrema, b200ldu_addr *a, int nLi
     }
     b200ldu_ctx *ctx = a->ctx;
     CUDA_TRY(cudaSetDevice(ctx->device));
-    cudaStream_t st = ctx->stream;
     const int n = a->nCells, nF = a->nFaces, nB = a->nBFaces;
     // scratch: psiMaxn, psiMinn, sumPhip, mSumPhim, lambdam, lambdap (six cell fields, kept across calls) + the received limiters
     double *psiMaxn = nullptr;
     TRY(a->mem.slot(ADDR_MULES, psiMaxn, (size_t)6 * n + (size_t)nCoupledFaces));
     double *psiMinn = psiMaxn + n, *sumPhip = psiMinn + n, *mSumPhim = sumPhip + n, *lambdam = mSumPhim + n,
            *lambdap = lambdam + n, *theirs = lambdap + n;
-    const int *bs = nB ? a->d_bCellStart : nullptr;
+    const fvmk::BoundaryLists L = boundary_lists(a);
     // lambda_d / lambdaB_d come in holding the starting limiter (MULES::limit: allLambda(mesh.nFaces(), 1.0))
-    mules_bounds_kernel<<<(n + 127) / 128, 128, 0, st>>>(n, a->d_ownerStart, a->d_u, a->d_losortStart, a->d_losort, a->d_l, bs,
-                                                         a->d_bCellFaces, psi_d, psiB_d, phiBD_d, phiBDB_d, phiCorr_d, phiCorrB_d,
-                                                         psi0_d, rho_d, rho0_d, Sp_d, Su_d, V_d, rDeltaT, psiMax, psiMin, psiMaxn,
-                                                         psiMinn, sumPhip, mSumPhim, corr, extrema);
-    ctx->launches++;
+    TRY(launch(ctx, mules_bounds_kernel, n, 128, n, a->d_ownerStart, a->d_u, a->d_losortStart, a->d_losort, a->d_l, L.bStart,
+               L.bFaces, psi_d, psiB_d, phiBD_d, phiBDB_d, phiCorr_d, phiCorrB_d, psi0_d, rho_d, rho0_d, Sp_d, Su_d, V_d, rDeltaT,
+               psiMax, psiMin, psiMaxn, psiMinn, sumPhip, mSumPhim, corr, extrema));
     for (int j = 0; j < nLimiterIter; j++) {
-        mules_cell_lambda_kernel<<<(n + 127) / 128, 128, 0, st>>>(n, a->d_ownerStart, a->d_losortStart, a->d_losort, bs,
-                                                                  a->d_bCellFaces, lambda_d, lambdaB_d, phiCorr_d, phiCorrB_d,
-                                                                  psiMaxn, psiMinn, sumPhip, mSumPhim, lambdam, lambdap);
-        mules_face_lambda_kernel<<<(nF + nB + 255) / 256, 256, 0, st>>>(nF, nB, nCoupledFaces, corr, a->d_l, a->d_u, a->d_bFaceCells, phiCorr_d,
-                                                                        phiCorrB_d, phiBDB_d, lambdam, lambdap, lambda_d,
-                                                                        lambdaB_d);
-        ctx->launches += 2;
+        TRY(launch(ctx, mules_cell_lambda_kernel, n, 128, n, a->d_ownerStart, a->d_losortStart, a->d_losort, L.bStart, L.bFaces,
+                   lambda_d, lambdaB_d, phiCorr_d, phiCorrB_d, psiMaxn, psiMinn, sumPhip, mSumPhim, lambdam, lambdap));
+        TRY(launch(ctx, mules_face_lambda_kernel, (long long)nF + nB, 256, nF, nB, nCoupledFaces, corr, a->d_l, a->d_u,
+                   a->d_bFaceCells, phiCorr_d, phiCorrB_d, phiBDB_d, lambdam, lambdap, lambda_d, lambdaB_d));
         if (nCoupledFaces) {
             double *mine = lambdaB_d + (nB - nCoupledFaces);
             TRY(comm_exchange_patch_field(a, 1, mine, theirs));
-            mules_sync_min_kernel<<<(nCoupledFaces + 255) / 256, 256, 0, st>>>(nCoupledFaces, mine, theirs);
-            ctx->launches++;
+            TRY(launch(ctx, mules_sync_min_kernel, nCoupledFaces, 256, nCoupledFaces, mine, theirs));
         }
     }
-    KERNEL_CHECK();
     return B200LDU_OK;
 }
 
