@@ -355,6 +355,33 @@ int b200ldu_fv_limiter(b200ldu_addr *a, const char *scheme, double k, const doub
 int b200ldu_fv_limited_weights(b200ldu_ctx *ctx, long long n, const double *limiter_d, const double *cdWeights_d,
                                const double *faceFlux_d, double *weights_d);
 
+/* ---- the face passes of the interFoam phase-fraction step (applications/solvers/multiphase/interFoam/alphaEqn.H,
+ * src/transportModels/interfaceProperties/interfaceProperties.C; sequenced by rapidcfd-dev_b200/interfoam.py) ----
+ * b200ldu_fv_limited_flux: flux_d[f] = outSign*(F*face) with F = fluxSign*faceFlux[f] and face the value of vf that the limited
+ *   scheme interpolates under F -- fvc::flux(F, vf, scheme) on the internal faces (gaussConvectionScheme.C:74-84) in one pass:
+ *   NVDTVD::r and the limiter as b200ldu_fv_limiter (same scheme names and k), w = lim*cdWeights + (1 - lim)*pos(F)
+ *   (limitedSurfaceInterpolationScheme.C:155-212), face = w*(vf[own] - vf[nei]) + vf[nei] (surfaceInterpolationScheme.C:272-351),
+ *   every operation rounded on its own: bit for bit b200ldu_fv_limiter -> _limited_weights -> _interpolate_linear ->
+ *   b200ldu_field_binary(mul), without their three face fields.  fluxSign, outSign: +1 or -1 (exact), so that
+ *   -fvc::flux(-phir, alpha2, scheme) (alphaEqn.H:92-97) is one call.  gradc_d = fvc::grad(vf) [3 per cell] and C_d = cell centres
+ *   [3 per cell] may be NULL for "upwind" and "linear".  Boundary faces are the caller's: faceFlux_b*vf_b.
+ * b200ldu_vof_interface_flux: interfaceProperties::calculateK up to nHatf (interfaceProperties.C:118-145) and the compression
+ *   flux.  Internal faces: gradAlphaf = w*(g[own] - g[nei]) + g[nei] per component of g = gradAlpha_d = fvc::grad(alpha1)
+ *   [3 per cell]; nHatfv = gradAlphaf/(mag(gradAlphaf) + deltaN), one division per component (VectorSpaceI.H:621-630), mag =
+ *   sqrt((x*x + y*y) + z*z); nHatf_d = (nHatfv.x*Sf.x + nHatfv.y*Sf.y) + nHatfv.z*Sf.z.  With phi_d != NULL also phir_d =
+ *   (cAlpha*|phi/magSf|)*nHatf (alphaEqn.H:6, :82); phi_d NULL: magSf_d, phir_d unused.  The non-coupled boundary faces of
+ *   b200ldu_fv_boundary_set: the face value of g is the cell value with its normal component replaced by the patch's snGrad,
+ *   g += n*(bSnGrad - (n & g)), n = bSf/mag(bSf) (gaussGrad.C:277-303); bSnGrad_d [nBFaces] is 0 for zeroGradient alpha1 and
+ *   deltaCoeffs*(alpha_b - alpha_c) for fixedValue; nHatfB_d [nBFaces] from it as on the internal faces.  phic is zero on
+ *   non-coupled boundary faces (alphaEqn.H:17-25), so phir has no boundary output.  No contact angles (correctContactAngle).
+ *   K = -fvc::div(nHatf) is b200ldu_fv_surface_integrate and a negation. */
+int b200ldu_fv_limited_flux(b200ldu_addr *a, const char *scheme, double k, const double *faceFlux_d, const double *vf_d,
+                            const double *gradc_d, const double *C_d, const double *cdWeights_d, int fluxSign, int outSign,
+                            double *flux_d);
+int b200ldu_vof_interface_flux(b200ldu_addr *a, const double *w_d, const double *gradAlpha_d, const double *Sf_d,
+                               const double *bSf_d, const double *bSnGrad_d, double deltaN, const double *phi_d,
+                               const double *magSf_d, double cAlpha, double *nHatf_d, double *nHatfB_d, double *phir_d);
+
 /* ---- structural self-check of the banded layout (host only, no GPU, no arithmetic);
  * used by the CPU test-suite.  what: 0 perm 1 iperm 2 sliceStart(int64) 3 sliceW(u16)
  * 4 sliceWL(u16) 5 col(u16) 6 code(int32) 7 haloStart 8 haloIdx 9 dims{nPad,nBands,bandRows,

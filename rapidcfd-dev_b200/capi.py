@@ -156,6 +156,8 @@ def lib():
     L.b200ldu_ldu_scale.argtypes = [vp, vp, C.c_double, vp, vp, vp, vp]
     L.b200ldu_fv_limiter.argtypes = [vp, C.c_char_p, C.c_double, vp, vp, vp, vp, vp]
     L.b200ldu_fv_limited_weights.argtypes = [vp, C.c_longlong, vp, vp, vp, vp]
+    L.b200ldu_fv_limited_flux.argtypes = [vp, C.c_char_p, C.c_double, vp, vp, vp, vp, vp, C.c_int, C.c_int, vp]
+    L.b200ldu_vof_interface_flux.argtypes = [vp] * 6 + [C.c_double, vp, vp, C.c_double, vp, vp, vp]
     L.b200ldu_field_binary.argtypes = [vp, C.c_int, C.c_longlong, C.c_int, vp, C.c_int, vp, vp]
     L.b200ldu_field_unary.argtypes = [vp, C.c_int, C.c_longlong, C.c_double, vp, vp]
     L.b200ldu_field_dot3.argtypes = [vp, C.c_longlong, vp, vp, vp]
@@ -681,6 +683,26 @@ def fv_limited_weights(ctx, faceFlux, limiter=None, cdWeights=None):
     out = _newlike(faceFlux, faceFlux.numel())
     check(lib().b200ldu_fv_limited_weights(ctx.h, faceFlux.numel(), _dp(limiter), _dp(cdWeights), _dp(faceFlux), _dp(out)))
     return out
+
+
+def fv_limited_flux(addr, scheme, faceFlux, vf, gradc, centres, cdWeights, k=1.0, fluxSign=1, outSign=1):
+    """outSign*fvc::flux(fluxSign*faceFlux, vf, scheme) on the internal faces in one pass: limiter, weights, face value and the
+    product with the flux, bit for bit the composition of fv_limiter, fv_limited_weights, fv_interpolate_linear and a multiply"""
+    out = _newlike(faceFlux, addr.nFaces)
+    check(lib().b200ldu_fv_limited_flux(addr.h, scheme.encode(), float(k), _dp(faceFlux), _dp(vf), _dp(gradc), _dp(centres),
+                                        _dp(cdWeights), int(fluxSign), int(outSign), _dp(out)))
+    return out
+
+
+def vof_interface_flux(addr, w, gradAlpha, Sf, bSf, bSnGrad, deltaN, phi=None, magSf=None, cAlpha=0.0):
+    """interfaceProperties::calculateK up to nHatf, and the compression flux: (nHatf on the internal faces, nHatf on the boundary
+    faces of fv_boundary_set, phir = cAlpha*|phi/magSf|*nHatf on the internal faces or None without phi)"""
+    nB = 0 if bSnGrad is None else bSnGrad.numel()
+    nHatf, nHatfB = _newlike(w, addr.nFaces), _newlike(w, max(nB, 1))
+    phir = None if phi is None else _newlike(w, addr.nFaces)
+    check(lib().b200ldu_vof_interface_flux(addr.h, _dp(w), _dp(gradAlpha), _dp(Sf), _dp(bSf), _dp(bSnGrad), float(deltaN), _dp(phi),
+                                           _dp(magSf), float(cAlpha), _dp(nHatf), _dp(nHatfB), _dp(phir)))
+    return nHatf, nHatfB[:nB], phir
 
 
 def mules_limiter(addr, V, rDeltaT, psi, psi0, psiB, phiBD, phiBDB, phiCorr, phiCorrB, psiMax, psiMin, nLimiterIter=3,

@@ -63,12 +63,8 @@ extern "C" int b200ldu_fv_sngrad(b200ldu_addr *a, int nComp, const double *delta
 }
 
 // ---- limited / upwind interpolation weights (SURVEY.md section 8(f) rank 1) ----
-// limiter field of a limited scheme on the internal faces (LimitedScheme.C:60-140); gradc = fvc::grad(vf) (b200ldu_fv_grad_linear),
-// C = cell centres.  scheme: "upwind" | "linear" | "limitedLinear" (coefficient k) | "vanLeer" | "Minmod"
-extern "C" int b200ldu_fv_limiter(b200ldu_addr *a, const char *scheme, double k, const double *faceFlux_d, const double *vf_d,
-                                  const double *gradc_d, const double *C_d, double *limiter_d)
+int limiter_scheme(const char *scheme, double k, int *code, double *twoByk)
 {
-    if (!a || !scheme || !limiter_d) return B200LDU_EINVAL;
     int sch;
     if (!strcmp(scheme, "upwind"))
         sch = LIM_UPWIND;
@@ -84,14 +80,28 @@ extern "C" int b200ldu_fv_limiter(b200ldu_addr *a, const char *scheme, double k,
         b200_set_error("Unknown discretisation scheme %s; valid schemes are: (Minmod limitedLinear linear upwind vanLeer)", scheme);
         return B200LDU_EINVAL;
     }
-    if (sch >= LIM_LIMITED_LINEAR && (!faceFlux_d || !vf_d || !gradc_d || !C_d)) return B200LDU_EINVAL;
     if (sch == LIM_LIMITED_LINEAR && (k < 0 || k > 1)) {
         b200_set_error("limitedLinear: coefficient = %g should be >= 0 and <= 1 (limitedLinear.H:66-72)", k);
         return B200LDU_EINVAL;
     }
-    CUDA_TRY(cudaSetDevice(a->ctx->device));
     const double kk = k > 1e-15 ? k : 1e-15;   // twoByk_ = 2.0/max(k_, SMALL), SMALL = 1e-15 (doubleScalar.H)
-    return launch(a->ctx, limiter_kernel, a->nFaces, 256, a->nFaces, sch, 2.0 / kk, a->d_l, a->d_u, faceFlux_d, vf_d, gradc_d,
+    *code = sch;
+    *twoByk = 2.0 / kk;
+    return B200LDU_OK;
+}
+
+// limiter field of a limited scheme on the internal faces (LimitedScheme.C:60-140); gradc = fvc::grad(vf) (b200ldu_fv_grad_linear),
+// C = cell centres.  scheme: "upwind" | "linear" | "limitedLinear" (coefficient k) | "vanLeer" | "Minmod"
+extern "C" int b200ldu_fv_limiter(b200ldu_addr *a, const char *scheme, double k, const double *faceFlux_d, const double *vf_d,
+                                  const double *gradc_d, const double *C_d, double *limiter_d)
+{
+    if (!a || !scheme || !limiter_d) return B200LDU_EINVAL;
+    int sch;
+    double twoByk;
+    TRY(limiter_scheme(scheme, k, &sch, &twoByk));
+    if (sch >= LIM_LIMITED_LINEAR && (!faceFlux_d || !vf_d || !gradc_d || !C_d)) return B200LDU_EINVAL;
+    CUDA_TRY(cudaSetDevice(a->ctx->device));
+    return launch(a->ctx, limiter_kernel, a->nFaces, 256, a->nFaces, sch, twoByk, a->d_l, a->d_u, faceFlux_d, vf_d, gradc_d,
                   C_d, limiter_d);
 }
 

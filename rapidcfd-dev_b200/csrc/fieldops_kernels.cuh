@@ -118,28 +118,30 @@ __device__ __forceinline__ double nvdtvd_r(double faceFlux, double phiP, double 
 // face from the scheme's limiter function -- upwind 0 (upwind.H:103-118), linear 1, limitedLinear
 // max(min(2/max(k,SMALL)*r, 1), 0) (limitedLinear.H:64-101), vanLeer (r + |r|)/(1 + |r|) (vanLeer.H:66-85),
 // Minmod max(min(r, 1), 0) (Minmod.H:66-85)
+__device__ __forceinline__ double face_limiter(int scheme, double twoByk, int o, int n, double faceFlux,
+                                               const double *__restrict__ vf, const double *__restrict__ gradc,
+                                               const double *__restrict__ C)
+{
+    if (scheme == LIM_UPWIND || scheme == LIM_LINEAR) return scheme == LIM_LINEAR ? 1.0 : 0.0;
+    const double d[3] = {__dsub_rn(C[3 * (size_t)n], C[3 * (size_t)o]), __dsub_rn(C[3 * (size_t)n + 1], C[3 * (size_t)o + 1]),
+                         __dsub_rn(C[3 * (size_t)n + 2], C[3 * (size_t)o + 2])};
+    const double r = nvdtvd_r(faceFlux, vf[o], vf[n], gradc + 3 * (size_t)o, gradc + 3 * (size_t)n, d);
+    if (scheme == LIM_LIMITED_LINEAR) return fmax(fmin(__dmul_rn(twoByk, r), 1.0), 0.0);
+    if (scheme == LIM_VANLEER) return __ddiv_rn(__dadd_rn(r, fabs(r)), __dadd_rn(1.0, fabs(r)));
+    return fmax(fmin(r, 1.0), 0.0);
+}
+
 __global__ void limiter_kernel(int nFaces, int scheme, double twoByk, const int *__restrict__ l, const int *__restrict__ u,
                                const double *__restrict__ faceFlux, const double *__restrict__ vf,
                                const double *__restrict__ gradc, const double *__restrict__ C, double *__restrict__ out)
 {
     const int f = blockIdx.x * blockDim.x + threadIdx.x;
     if (f >= nFaces) return;
-    if (scheme == LIM_UPWIND || scheme == LIM_LINEAR) {
+    if (scheme == LIM_UPWIND || scheme == LIM_LINEAR) { // neither reads its arguments, which may be NULL
         out[f] = scheme == LIM_LINEAR ? 1.0 : 0.0;
         return;
     }
-    const int o = l[f], n = u[f];
-    const double d[3] = {__dsub_rn(C[3 * (size_t)n], C[3 * (size_t)o]), __dsub_rn(C[3 * (size_t)n + 1], C[3 * (size_t)o + 1]),
-                         __dsub_rn(C[3 * (size_t)n + 2], C[3 * (size_t)o + 2])};
-    const double r = nvdtvd_r(faceFlux[f], vf[o], vf[n], gradc + 3 * (size_t)o, gradc + 3 * (size_t)n, d);
-    double lim;
-    if (scheme == LIM_LIMITED_LINEAR)
-        lim = fmax(fmin(__dmul_rn(twoByk, r), 1.0), 0.0);
-    else if (scheme == LIM_VANLEER)
-        lim = __ddiv_rn(__dadd_rn(r, fabs(r)), __dadd_rn(1.0, fabs(r)));
-    else
-        lim = fmax(fmin(r, 1.0), 0.0);
-    out[f] = lim;
+    out[f] = face_limiter(scheme, twoByk, l[f], u[f], faceFlux[f], vf, gradc, C);
 }
 
 // limitedSurfaceInterpolationScheme::weights (limitedSurfaceInterpolationScheme.C:155-212):

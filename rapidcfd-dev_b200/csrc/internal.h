@@ -349,6 +349,10 @@ struct b200ldu_matrix {
 // ---------------------------------------------------------------------------
 int layout_build(b200ldu_addr *a, const double *centres);
 
+// a limited scheme's name and coefficient as the kernels take them (fieldops.cu): the fieldk::LIM_* code and
+// 2/max(k, SMALL); an unknown name or a limitedLinear coefficient outside [0, 1] is B200LDU_EINVAL with the reference's message
+int limiter_scheme(const char *scheme, double k, int *code, double *twoByk);
+
 // banded vector of a's vecLen doubles in slot k of mem, zeroed when first allocated (its padding rows and receive tail
 // rely on it); nullptr when the allocation fails
 inline double *banded_vec(const b200ldu_addr *a, DeviceMem &mem, int k)

@@ -371,6 +371,25 @@ def convection_scheme(tokens):
     return name, k, bounded
 
 
+def alpha_controls(fvSolution, fvSchemes, fieldName="alpha.water"):
+    """The controls of the interFoam phase-fraction step (rapidcfd-dev_b200/interfoam.py) from the `fieldName` solver entry of an
+    fvSolution FoamDict and an FvSchemes, as FV/cfdTools/general/include/alphaControls.H, interfaceProperties.C:172-178 and MULES
+    read them: nAlphaCorr, nAlphaSubCycles and cAlpha are required; MULESCorr and alphaApplyPrevCorr default to false, icAlpha to
+    0; with MULESCorr, nLimiterIter is required (CMULESTemplates.C:95-98) and extremaCoeff defaults to 0 (:398-401) -- the explicit
+    MULES::explicitSolve always sweeps three times (MULESTemplates.C:113).  alphaScheme / alpharScheme: (scheme word, k) of the
+    divSchemes entries div(phi,alpha) / div(phirb,alpha); a scheme the limiter does not know is refused by name."""
+    sd = fvSolution.subDict("solvers").subDict(fieldName)
+    c = dict(nAlphaCorr=int(sd.lookup("nAlphaCorr")), nAlphaSubCycles=int(sd.lookup("nAlphaSubCycles")), cAlpha=float(sd.lookup("cAlpha")),
+             MULESCorr=bool(_switch(sd.lookupOrDefault("MULESCorr", "no"))),
+             alphaApplyPrevCorr=bool(_switch(sd.lookupOrDefault("alphaApplyPrevCorr", "no"))), icAlpha=float(sd.lookupOrDefault("icAlpha", 0)),
+             nLimiterIter=3, extremaCoeff=float(sd.lookupOrDefault("extremaCoeff", 0.0)))
+    if c["MULESCorr"]:
+        c["nLimiterIter"] = int(sd.lookup("nLimiterIter"))
+    for key, name in (("alphaScheme", "div(phi,alpha)"), ("alpharScheme", "div(phirb,alpha)")):
+        c[key] = convection_scheme(fvSchemes.div(name))[:2]
+    return c
+
+
 # ---------------------------------------------------------------------------
 # FoamFile list files
 # ---------------------------------------------------------------------------
