@@ -7,7 +7,7 @@ name=$1; shift
 cd "$(dirname "$0")/../rapidcfd-dev_b200/csrc"
 mkdir -p build_$name
 NV="/usr/local/cuda/bin/nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -lineinfo --extended-lambda -Xcompiler -fPIC,-fopenmp,-Wall,-Wno-unused-function -ccbin /usr/bin/g++"
-for f in ldu layout comm solvers gamg fv fvmatrix fieldops lduops mules; do
+for f in ldu layout comm solvers gamg fv fvmatrix fieldops lduops mules vof; do
   $NV "$@" -c -o build_$name/$f.o $f.cu &
 done
 wait
