@@ -161,7 +161,8 @@ int b200ldu_smooth(b200ldu_matrix *m, const char *name, double omega, double *ps
                    const double *source_d, int nSweeps);
 
 /* banded-order views for benchmarking the kernels exactly as the solvers run them:
- * vectors of b200ldu_vec_len() doubles in banded row order (+ halo tail). */
+ * vectors of b200ldu_vec_len() doubles in banded row order (+ halo tail).  amul_banded exchanges the coupled-patch
+ * values into the halo tail of psib (doubles [nPad, vec_len)) before the product: only its rows are read-only. */
 long long b200ldu_vec_len(const b200ldu_addr *a);
 int b200ldu_to_banded(b200ldu_addr *a, const double *x_d, double *xb_d);
 int b200ldu_from_banded(b200ldu_addr *a, const double *xb_d, double *x_d);
@@ -292,8 +293,10 @@ int b200ldu_fvm_solve(b200ldu_matrix *m, int nComp, const char *solver, const ch
  * caller that composes them in the reference's order reproduces the reference's field expressions.  n = elements;
  * a 1-component operand combines with a 3-component one component-wise (scalargpuField * vectorgpuField).
  *   binary op: 0 a+b, 1 a-b, 2 a*b, 3 a/b, 4 min(a,b), 5 max(a,b)
- *   unary  op (n = number of doubles): 0 -a, 1 |a|, 2 s*a, 3 s/a, 4 a+s, 5 s-a, 6 min(a,s), 7 max(a,s), 8 a-s, 9 a/s, 10 a
- *   dot3: (a.x*b.x + a.y*b.y) + a.z*b.z per element;  gather: patchInternalField, out[i] = field[cells[i]] */
+ *   unary  op (n = number of doubles): 0 -a, 1 |a|, 2 s*a, 3 s/a, 4 a+s, 5 s-a, 6 min(a,s), 7 max(a,s), 8 a-s, 9 a/s, 10 a,
+ *     11 pos(a) (1 where a >= 0, else 0)
+ *   dot3: (a.x*b.x + a.y*b.y) + a.z*b.z per element;  gather: patchInternalField, out[i] = field[cells[i]]
+ *   With n = 0 the arrays may be NULL (an empty field hands out no pointer). */
 int b200ldu_field_binary(b200ldu_ctx *ctx, int op, long long n, int nCompA, const double *a_d, int nCompB,
                          const double *b_d, double *out_d);
 int b200ldu_field_unary(b200ldu_ctx *ctx, int op, long long n, double s, const double *a_d, double *out_d);

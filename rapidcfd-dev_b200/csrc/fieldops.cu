@@ -17,7 +17,7 @@ using namespace fieldk;
 extern "C" int b200ldu_field_binary(b200ldu_ctx *ctx, int op, long long n, int ncA, const double *a_d, int ncB,
                                     const double *b_d, double *out_d)
 {
-    if (!ctx || !a_d || !b_d || !out_d || n < 0 || op < OP_ADD || op > OP_MAX) return B200LDU_EINVAL;
+    if (!ctx || (n && (!a_d || !b_d || !out_d)) || n < 0 || op < OP_ADD || op > OP_MAX) return B200LDU_EINVAL;
     if ((ncA != 1 && ncA != 3) || (ncB != 1 && ncB != 3)) return B200LDU_EINVAL;
     CUDA_TRY(cudaSetDevice(ctx->device));
     const int nc = ncA > ncB ? ncA : ncB;
@@ -26,21 +26,21 @@ extern "C" int b200ldu_field_binary(b200ldu_ctx *ctx, int op, long long n, int n
 
 extern "C" int b200ldu_field_unary(b200ldu_ctx *ctx, int op, long long n, double s, const double *a_d, double *out_d)
 {
-    if (!ctx || !a_d || !out_d || n < 0 || op < UN_NEG || op > UN_POS) return B200LDU_EINVAL;
+    if (!ctx || (n && (!a_d || !out_d)) || n < 0 || op < UN_NEG || op > UN_POS) return B200LDU_EINVAL;
     CUDA_TRY(cudaSetDevice(ctx->device));
     return launch(ctx, unary_kernel, n, 256, n, op, s, a_d, out_d);
 }
 
 extern "C" int b200ldu_field_dot3(b200ldu_ctx *ctx, long long n, const double *a_d, const double *b_d, double *out_d)
 {
-    if (!ctx || !a_d || !b_d || !out_d || n < 0) return B200LDU_EINVAL;
+    if (!ctx || (n && (!a_d || !b_d || !out_d)) || n < 0) return B200LDU_EINVAL;
     CUDA_TRY(cudaSetDevice(ctx->device));
     return launch(ctx, dot3_kernel, n, 256, n, a_d, b_d, out_d);
 }
 
 extern "C" int b200ldu_field_symm_magsqr(b200ldu_ctx *ctx, long long n, const double *tensor_d, double *out_d)
 {
-    if (!ctx || !tensor_d || !out_d || n < 0) return B200LDU_EINVAL;
+    if (!ctx || (n && (!tensor_d || !out_d)) || n < 0) return B200LDU_EINVAL;
     CUDA_TRY(cudaSetDevice(ctx->device));
     return launch(ctx, symm_magsqr_kernel, n, 256, n, tensor_d, out_d);
 }
@@ -48,7 +48,7 @@ extern "C" int b200ldu_field_symm_magsqr(b200ldu_ctx *ctx, long long n, const do
 extern "C" int b200ldu_field_gather(b200ldu_ctx *ctx, int n, int nComp, const int *cells_d, const double *field_d,
                                     double *out_d)
 {
-    if (!ctx || !cells_d || !field_d || !out_d || n < 0 || (nComp != 1 && nComp != 3)) return B200LDU_EINVAL;
+    if (!ctx || (n && (!cells_d || !field_d || !out_d)) || n < 0 || (nComp != 1 && nComp != 3)) return B200LDU_EINVAL;
     CUDA_TRY(cudaSetDevice(ctx->device));
     return launch(ctx, gather_kernel, (long long)n * nComp, 256, n, nComp, cells_d, field_d, out_d);
 }

@@ -84,7 +84,6 @@ struct b200ldu_gamg {
     std::vector<int> coarsestCounts, coarsestOffs, coarsestNbrCell;
     int nMaxCoarsest = 0;
     double *d_gatherAll = nullptr; // NCCL fallback of the peer-memory gather
-    bool metaUploaded = false;
 };
 
 // ---------------------------------------------------------------------------
@@ -842,9 +841,17 @@ static int gamg_coarsest_inverse(Solve &S, b200ldu_gamg *g)
     TRY(g->mem.slot(GAMG_INV, g->d_inv, (size_t)std::max(n, 1) * N));
     g->invN = N;
     CUDA_TRY(cudaMemcpyAsync(g->d_inv, &I[(size_t)off * N], sizeof(double) * (size_t)n * N, cudaMemcpyHostToDevice, st));
-    if (R > 1 && !ctx->p2p) // the gathered right-hand sides, then 64 ints of rank offsets and counts
+    std::vector<int> meta(64, 0);
+    if (R > 1 && !ctx->p2p) {
+        // the gathered right-hand sides, then 64 ints of rank offsets and counts.  The ints live in a double slot, so
+        // they are written here, after every allocation of it, and never rely on what a new block holds
         TRY(g->mem.slot(GAMG_GATHER, g->d_gatherAll, (size_t)(R + 1) * P2P_GMAX + 32));
-    CUDA_TRY(cudaStreamSynchronize(st)); // I goes out of scope
+        for (int r = 0; r <= R; r++) meta[r] = g->coarsestOffs[r];
+        for (int r = 0; r < R; r++) meta[32 + r] = g->coarsestCounts[r];
+        CUDA_TRY(cudaMemcpyAsync(g->d_gatherAll + (size_t)(R + 1) * P2P_GMAX, meta.data(), sizeof(int) * 64,
+                                 cudaMemcpyHostToDevice, st));
+    }
+    CUDA_TRY(cudaStreamSynchronize(st)); // I and meta go out of scope
     return B200LDU_OK;
 }
 
@@ -909,15 +916,7 @@ static int gamg_cycle(Solve &S, b200ldu_gamg *g, int scaleCorrection, double *co
                 CUDA_TRY(cudaMemsetAsync(mine, 0, sizeof(double) * P2P_GMAX, st));
                 CUDA_TRY(cudaMemcpyAsync(mine, L.src, sizeof(double) * L.nCoarse, cudaMemcpyDeviceToDevice, st));
                 TRY(comm_allgather_dev(S.ctx, mine, P2P_GMAX, g->d_gatherAll));
-                int *meta = (int *)(g->d_gatherAll + (size_t)(S.ctx->nRanks + 1) * P2P_GMAX);
-                if (!g->metaUploaded) {
-                    std::vector<int> h(64, 0);
-                    for (int r = 0; r <= S.ctx->nRanks; r++) h[r] = g->coarsestOffs[r];
-                    for (int r = 0; r < S.ctx->nRanks; r++) h[32 + r] = g->coarsestCounts[r];
-                    CUDA_TRY(cudaMemcpyAsync(meta, h.data(), sizeof(int) * 64, cudaMemcpyHostToDevice, st));
-                    CUDA_TRY(cudaStreamSynchronize(st));
-                    g->metaUploaded = true;
-                }
+                const int *meta = (const int *)(g->d_gatherAll + (size_t)(S.ctx->nRanks + 1) * P2P_GMAX);
                 dense_apply_gathered_kernel<<<1, 256, 0, st>>>(L.nCoarse, g->invN, S.ctx->nRanks, g->d_inv, g->d_gatherAll,
                                                                 meta, meta + 32, L.corr, stop);
             }

@@ -64,12 +64,16 @@ struct b200ldu_ctx {
     unsigned long long *d_seq = nullptr; // local device counters: [0] reduction seq, [1] halo seq, [2..] scratch
     // device memory of the handles created on this context (DeviceMem): bytes held, allocations made
     long long memLive = 0, memAllocs = 0;
+    // B200LDU_POISON_ALLOC, read by ctx_create: DeviceMem fills every new floating-point block that is not zeroNew with
+    // byte 0xFF (a NaN per double), so that a result that depends on memory nobody wrote shows
+    bool poison = false;
 };
 
 // Device memory of one handle (addressing, matrix, GAMG hierarchy): every device array the handle holds is allocated
 // here and freed with the handle.  Fixed arrays live as long as the handle; numbered slots grow on demand and never
 // shrink.  The contents of a slot are unspecified after it was reallocated, except that zeroNew zeroes a new
-// allocation on the context's stream.
+// allocation on the context's stream.  On a poisoning context (b200ldu_ctx::poison) a new floating-point block that is
+// not zeroNew holds NaNs (byte 0xFF) instead; integer and flag arrays are never poisoned.
 class DeviceMem {
   public:
     explicit DeviceMem(b200ldu_ctx *ctx) : ctx_(ctx) {}
@@ -131,7 +135,13 @@ class DeviceMem {
             b.bytes = bytes;
             ctx_->memLive += (long long)bytes;
             ctx_->memAllocs++;
-            if (zeroNew) CUDA_TRY(cudaMemsetAsync(b.p, 0, bytes, ctx_->stream));
+            if (zeroNew) {
+                CUDA_TRY(cudaMemsetAsync(b.p, 0, bytes, ctx_->stream));
+            } else if (std::is_floating_point<T>::value && ctx_->poison) {
+                // synchronised: an upload (copy_in) is not ordered after work on the context's stream
+                CUDA_TRY(cudaMemsetAsync(b.p, 0xFF, bytes, ctx_->stream));
+                CUDA_TRY(cudaStreamSynchronize(ctx_->stream));
+            }
         }
         d = (T *)b.p;
         return B200LDU_OK;

@@ -72,6 +72,8 @@ extern "C" int b200ldu_ctx_create(int device, b200ldu_ctx **out)
     c->smCount = p.multiProcessorCount;
     CUDA_TRY(cudaStreamCreateWithFlags(&c->ownStream, cudaStreamNonBlocking));
     c->stream = c->ownStream;
+    const char *poison = getenv("B200LDU_POISON_ALLOC");
+    c->poison = poison && *poison && strcmp(poison, "0") != 0;
     CUDA_TRY(cudaMallocHost(&c->pinned, sizeof(PinnedArea)));
     *out = c;
     return B200LDU_OK;
