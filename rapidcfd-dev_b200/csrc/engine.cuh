@@ -37,6 +37,11 @@ __device__ __forceinline__ uint32_t ldg_stream_u32(const void *p)
     return r;
 }
 
+__device__ __forceinline__ void prefetch_l2(const void *p)
+{
+    asm volatile("prefetch.global.L2 [%0];" ::"l"(p));
+}
+
 __device__ __forceinline__ void cp_async16(void *smemDst, const void *gsrc)
 {
     unsigned d = (unsigned)__cvta_generic_to_shared(smemDst);
@@ -129,11 +134,27 @@ __host__ __device__ __forceinline__ bool fused_pack(const Op &op, const LayoutDe
     return Op::STAGED && !Op::LOCAL && op.waitHalo && L.nPackChunks > 0;
 }
 
+// Predicated loads for the face stream's owner slots: when `pred` is false nothing is read (the address may lie past the
+// stream) and the result is zero.  Setting the result before the predicated load ends its live range there, so a
+// partial group neither keeps the previous group's registers alive nor needs a branch around its loads.
+__device__ __forceinline__ double2 ldg_stream2_if(bool pred, const double *p)
+{
+    double2 r;
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %2, 0;\n\tmov.b64 %0, 0;\n\tmov.b64 %1, 0;\n\t"
+                 "@p ld.global.nc.L1::no_allocate.v2.f64 {%0, %1}, [%3];\n\t}"
+                 : "=d"(r.x), "=d"(r.y)
+                 : "r"((int)pred), "l"(p));
+    return r;
+}
+
 // the face stream's words come from a small table that many slices share: keep them in L1
-__device__ __forceinline__ uint2 ldg_table_u64(const void *p)
+__device__ __forceinline__ uint2 ldg_table_u64_if(bool pred, const void *p)
 {
     uint2 r;
-    asm volatile("ld.global.nc.v2.u32 {%0, %1}, [%2];" : "=r"(r.x), "=r"(r.y) : "l"(p));
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %2, 0;\n\tmov.b32 %0, 0;\n\tmov.b32 %1, 0;\n\t"
+                 "@p ld.global.nc.v2.u32 {%0, %1}, [%3];\n\t}"
+                 : "=r"(r.x), "=r"(r.y)
+                 : "r"((int)pred), "l"(p));
     return r;
 }
 
@@ -147,6 +168,10 @@ __device__ __forceinline__ double fs_owner(const Op &op, const double *xs, doubl
     if (t < FS_PAD) buf[t] = op.prod(v, aOwn);
     return acc;
 }
+
+// Owner slots per load group of the face stream's pass 1.  A hex mesh stores 3 owner faces per row, so one group covers
+// nearly every slice; a group of 4 would need registers that __launch_bounds__(256, 6) leaves only by spilling.
+constexpr int FS_GROUP = 3;
 
 template <class Op, bool FS>
 __global__ void __launch_bounds__(ENGINE_THREADS, 6) engine_kernel(const LayoutDev L, const double *__restrict__ val, Op op)
@@ -188,6 +213,16 @@ __global__ void __launch_bounds__(ENGINE_THREADS, 6) engine_kernel(const LayoutD
     const int rowBase = band * L.bandRows;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     constexpr int NW = ENGINE_THREADS / 32;
+
+    // Face stream: the slice descriptors and the band's list header are first read after the staging barrier, and from
+    // HBM (they are streamed once per sweep).  Prefetching them into L2 now, before staging, shortens the chain of
+    // memory round trips that pass 1 waits on without holding a register across the staging phase.
+    if (FS) {
+        if (lane == 0 && warp < L.slicesPerBand) prefetch_l2(L.fsSlice + band * L.slicesPerBand + warp);
+        if (tid == 32) prefetch_l2(L.fsListStart + band);
+        if (tid == 64) prefetch_l2(Op::LOCAL ? L.fsListIfc + band : L.fsListStart + band + 1);
+        if (tid == 96) prefetch_l2(L.fsListTpl + band);
+    }
 
     // ---- phase 1: stage the band's vector tile + halo ----
     double *const buf = xs + (Op::STAGED ? ((L.bandRows + L.maxHalo + 1) & ~1) : 0); // face stream: product buffer
@@ -235,26 +270,26 @@ __global__ void __launch_bounds__(ENGINE_THREADS, 6) engine_kernel(const LayoutD
             // 32-bit offsets of the lane's first slot, advanced slot by slot: the layout keeps the coefficient stream and
             // the template table below 2^31 entries (fsFits)
             unsigned vo = S.start64 * SLICE_ROWS + 2 * lane, co = S.tpl64 * SLICE_ROWS + 2 * lane;
-            int n = S.wo;
-            for (; n >= 4; n -= 4, vo += 4 * SLICE_ROWS, co += 4 * SLICE_ROWS) {
-                double2 v[4];
-                uint2 c[4];
+            // slots in groups of FS_GROUP, the last one guarded by k < n: all loads of a group are issued before any use, so
+            // a slice of 3 owner slots waits for one memory round trip, not three.  The uses follow in slot order, under
+            // the same guard.  The own-row values are read again from the tile, which pass 1 does not write: keeping
+            // them in registers across the group's loads would spill.
+#pragma unroll 1
+            for (int n = S.wo; n > 0; n -= FS_GROUP, vo += FS_GROUP * SLICE_ROWS, co += FS_GROUP * SLICE_ROWS) {
+                double2 v[FS_GROUP];
+                uint2 c[FS_GROUP];
 #pragma unroll
-                for (int k = 0; k < 4; k++) {
-                    v[k] = ldg_stream2(val + (vo + k * SLICE_ROWS));
-                    c[k] = ldg_table_u64(L.fsTpl + (co + k * SLICE_ROWS));
+                for (int k = 0; k < FS_GROUP; k++) {
+                    v[k] = ldg_stream2_if(k < n, val + (vo + k * SLICE_ROWS));
+                    c[k] = ldg_table_u64_if(k < n, L.fsTpl + (co + k * SLICE_ROWS));
                 }
+                const double2 a = Op::STAGED ? reinterpret_cast<const double2 *>(xs)[lr >> 1] : make_double2(0, 0);
 #pragma unroll
-                for (int k = 0; k < 4; k++) {
-                    acc0 = fs_owner(op, xs, buf, acc0, v[k].x, c[k].x, a0);
-                    acc1 = fs_owner(op, xs, buf, acc1, v[k].y, c[k].y, a1);
-                }
-            }
-            for (; n > 0; n--, vo += SLICE_ROWS, co += SLICE_ROWS) {
-                double2 v = ldg_stream2(val + vo);
-                uint2 c = ldg_table_u64(L.fsTpl + co);
-                acc0 = fs_owner(op, xs, buf, acc0, v.x, c.x, a0);
-                acc1 = fs_owner(op, xs, buf, acc1, v.y, c.y, a1);
+                for (int k = 0; k < FS_GROUP; k++)
+                    if (k < n) {
+                        acc0 = fs_owner(op, xs, buf, acc0, v[k].x, c[k].x, a.x);
+                        acc1 = fs_owner(op, xs, buf, acc1, v[k].y, c[k].y, a.y);
+                    }
             }
             reinterpret_cast<double2 *>(buf + S.bufOff)[lane] = make_double2(acc0, acc1);
         }
