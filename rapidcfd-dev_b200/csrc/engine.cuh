@@ -173,16 +173,40 @@ __device__ __forceinline__ double fs_owner(const Op &op, const double *xs, doubl
 // nearly every slice; a group of 4 would need registers that __launch_bounds__(256, 6) leaves only by spilling.
 constexpr int FS_GROUP = 3;
 
+// Halo columns per thread taken in one load group by the staging phase: every index load of the group is issued, then
+// every gather, then the shared-memory stores.  A 512-row band of a hex mesh has about 400 halo columns, so one group of 2
+// covers it; the rest, if any, follow one column at a time.
+constexpr int HALO_GROUP = 2;
+
 template <class Op, bool FS>
 __global__ void __launch_bounds__(ENGINE_THREADS, 6) engine_kernel(const LayoutDev L, const double *__restrict__ val, Op op)
 {
     extern __shared__ double xs[];
-    if (!op.prologue(L)) return; // stop flag (OpBase) or the deferred scalar step of the fused PCG (ops.cuh)
     // Fused halo send: the first nPackChunks CTAs of the grid gather the staged vector
     // at the processor-patch face cells, store it straight into the neighbours' receive
     // buffers over NVLink and release their arrival flags; all other CTAs are SpMV bands
     // (those that reference received values wait for the neighbours' flags below).
     const bool fusedPack = fused_pack(op, L);
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+
+    // Layout words that the staging phase and pass 1 read first are streamed once per sweep, so they come from HBM.
+    // None of them depends on the scalars that the prologue waits for: prefetching them into L2 now, while the prologue
+    // waits, takes their round trips off the chain the band waits on, without holding a register across it.  The face
+    // stream's slice descriptors and list header; the band's halo range and, one 128-byte line per lane, its halo indices.
+    if (const int band = blockIdx.x - (fusedPack ? L.nPackChunks : 0); band >= 0) {
+        if (FS) {
+            if (lane == 0 && warp < L.slicesPerBand) prefetch_l2(L.fsSlice + band * L.slicesPerBand + warp);
+            if (tid == 32) prefetch_l2(L.fsListStart + band);
+            if (tid == 64) prefetch_l2(Op::LOCAL ? L.fsListIfc + band : L.fsListStart + band + 1);
+            if (tid == 96) prefetch_l2(L.fsListTpl + band);
+        }
+        if (Op::STAGED && warp == 4) { // warp 0 waits on the gate, warps 0-3 prefetch the face stream's words
+            const int hs = __ldg(L.haloStart + band), hn = __ldg(L.haloStart + band + 1) - hs;
+            if (32 * lane < hn) prefetch_l2(L.haloIdx + hs + 32 * lane); // the first 1024 columns: a hint, not a copy
+            if (lane == 0 && hn > 0 && hn <= 1024) prefetch_l2(L.haloIdx + hs + hn - 1);
+        }
+    }
+    if (!op.prologue(L)) return; // stop flag (OpBase) or the deferred scalar step of the fused PCG (ops.cuh)
     unsigned long long haloSeqNow = 0;
     if (fusedPack) {
         haloSeqNow = L.seqs[1] + 1; // seqs[1] only advances when the whole grid has finished
@@ -211,26 +235,17 @@ __global__ void __launch_bounds__(ENGINE_THREADS, 6) engine_kernel(const LayoutD
     }
     const int band = blockIdx.x - (fusedPack ? L.nPackChunks : 0);
     const int rowBase = band * L.bandRows;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     constexpr int NW = ENGINE_THREADS / 32;
 
-    // Face stream: the slice descriptors and the band's list header are first read after the staging barrier, and from
-    // HBM (they are streamed once per sweep).  Prefetching them into L2 now, before staging, shortens the chain of
-    // memory round trips that pass 1 waits on without holding a register across the staging phase.
-    if (FS) {
-        if (lane == 0 && warp < L.slicesPerBand) prefetch_l2(L.fsSlice + band * L.slicesPerBand + warp);
-        if (tid == 32) prefetch_l2(L.fsListStart + band);
-        if (tid == 64) prefetch_l2(Op::LOCAL ? L.fsListIfc + band : L.fsListStart + band + 1);
-        if (tid == 96) prefetch_l2(L.fsListTpl + band);
-    }
-
     // ---- phase 1: stage the band's vector tile + halo ----
+    // The own rows first (stage_own issues its loads before it stores a fused vector update), then the band's halo range
+    // and its first group of indices, which the prefetch above has brought into L2, then the group's gathers, all issued
+    // before any of them is used.  The halo range is loaded after the own rows: held across them, it spilled.
     double *const buf = xs + (Op::STAGED ? ((L.bandRows + L.maxHalo + 1) & ~1) : 0); // face stream: product buffer
     if (Op::STAGED) {
-    for (int i = tid; i < (L.bandRows >> 1); i += ENGINE_THREADS)
-        reinterpret_cast<double2 *>(xs)[i] = op.stage_own(rowBase + 2 * i);
-    {
-        const int hs = L.haloStart[band], hn = L.haloStart[band + 1] - hs;
+        for (int i = tid; i < (L.bandRows >> 1); i += ENGINE_THREADS)
+            reinterpret_cast<double2 *>(xs)[i] = op.stage_own(rowBase + 2 * i);
+        const int hs = __ldg(L.haloStart + band), hn = __ldg(L.haloStart + band + 1) - hs;
         // peer-memory halo: bands that reference received values wait for the neighbours'
         // arrival flags here, so interior bands overlap with the exchange
         const double *remoteTail = nullptr;
@@ -242,11 +257,22 @@ __global__ void __launch_bounds__(ENGINE_THREADS, 6) engine_kernel(const LayoutD
                 __syncthreads();
             }
         }
-        for (int i = tid; i < hn; i += ENGINE_THREADS) {
-            int g = __ldg(L.haloIdx + hs + i);
-            xs[L.bandRows + i] = (remoteTail && g >= L.nPad) ? __ldcg(remoteTail + (g - L.nPad)) : op.stage(g);
+        if (!remoteTail) {
+            int g[HALO_GROUP];
+            double h[HALO_GROUP];
+#pragma unroll
+            for (int k = 0; k < HALO_GROUP; k++)
+                g[k] = tid + k * ENGINE_THREADS < hn ? __ldg(L.haloIdx + hs + tid + k * ENGINE_THREADS) : 0;
+#pragma unroll
+            for (int k = 0; k < HALO_GROUP; k++) h[k] = op.stage(g[k]); // row 0 past the halo: read, never stored
+#pragma unroll
+            for (int k = 0; k < HALO_GROUP; k++)
+                if (tid + k * ENGINE_THREADS < hn) xs[L.bandRows + tid + k * ENGINE_THREADS] = h[k];
         }
-    }
+        for (int i = remoteTail ? tid : tid + HALO_GROUP * ENGINE_THREADS; i < hn; i += ENGINE_THREADS) {
+            const int gi = __ldg(L.haloIdx + hs + i);
+            xs[L.bandRows + i] = (remoteTail && gi >= L.nPad) ? __ldcg(remoteTail + (gi - L.nPad)) : op.stage(gi);
+        }
     }
     if (FS) {
         const double e = op.identity();

@@ -394,22 +394,25 @@ struct PcgAinvOp : OpBase {
     const SolverScalars *sc;
     Pre pre; // scalar step of the previous sweep, run in this kernel's prologue
     __device__ __forceinline__ bool prologue(const LayoutDev &) const { return pre.run(); }
+    // the loads of stage() do not depend on one another: the engine issues a whole group of them before any use
     __device__ __forceinline__ double stage(int g) const
     {
-        double r = sc->bodies > 0 ? fma(-sc->alpha, w[g], rOld[g]) : rOld[g];
-        return __dmul_rn(rD[g], r);
+        const double ro = rOld[g], ww = w[g], d = rD[g];
+        const double r = sc->bodies > 0 ? fma(-sc->alpha, ww, ro) : ro;
+        return __dmul_rn(d, r);
     }
     __device__ __forceinline__ double2 stage_own(int row) const
     {
+        // rD is loaded before the store of rNew, which the compiler may not move a load past
         double2 r = *reinterpret_cast<const double2 *>(rOld + row);
+        const double2 ww = *reinterpret_cast<const double2 *>(w + row);
+        const double2 dd = *reinterpret_cast<const double2 *>(rD + row);
         if (sc->bodies > 0) {
             const double alpha = sc->alpha;
-            double2 ww = *reinterpret_cast<const double2 *>(w + row);
             r.x = fma(-alpha, ww.x, r.x);
             r.y = fma(-alpha, ww.y, r.y);
         }
         *reinterpret_cast<double2 *>(rNew + row) = r;
-        double2 dd = *reinterpret_cast<const double2 *>(rD + row);
         return make_double2(__dmul_rn(dd.x, r.x), __dmul_rn(dd.y, r.y));
     }
     __device__ __forceinline__ double init(int, double) const { return 0.0; }
@@ -438,20 +441,21 @@ struct PcgAmulOp : AmulOp<AMUL_OUT_X> {
     const SolverScalars *sc;
     Pre pre; // scalar step of the previous sweep, run in this kernel's prologue
     __device__ __forceinline__ bool prologue(const LayoutDev &) const { return pre.run(); }
+    // the loads of stage() do not depend on one another: the engine issues a whole group of them before any use
     __device__ __forceinline__ double stage(int g) const
     {
-        return sc->bodies == 0 ? z[g] : fma(sc->beta, pOld[g], z[g]);
+        const double zz = z[g], po = pOld[g];
+        return sc->bodies == 0 ? zz : fma(sc->beta, po, zz);
     }
     __device__ __forceinline__ double2 stage_own(int row) const
     {
         // every load before the first store (the compiler may not move a load past a store to a vector that could
-        // alias it): one memory round trip per row pair, not two.  Costs one 8-byte spill outside the loops; the
-        // sweep is 1 % faster for it (DESIGN §4)
+        // alias it): one memory round trip per row pair, not two (DESIGN §4)
         double2 zz = *reinterpret_cast<const double2 *>(z + row);
+        const double2 po = *reinterpret_cast<const double2 *>(pOld + row);
+        double2 x = *reinterpret_cast<const double2 *>(psi + row);
         if (sc->bodies > 0) {
             const double alpha = sc->alpha, beta = sc->beta;
-            const double2 po = *reinterpret_cast<const double2 *>(pOld + row);
-            double2 x = *reinterpret_cast<const double2 *>(psi + row);
             zz.x = fma(beta, po.x, zz.x);
             zz.y = fma(beta, po.y, zz.y);
             x.x = fma(alpha, po.x, x.x);
