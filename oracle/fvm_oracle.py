@@ -30,6 +30,19 @@ Findings while restating (mirrored, not corrected; both reproduced by running th
 import numpy as np
 
 
+def max_(s1, s2):
+    """max of two scalars as the reference defines it (label.H:285-297, instantiated for doubles by doubleFloat.H:69-86):
+    (s1 > s2) ? s1 : s2 -- the second operand on a tie (max(+0, -0) = -0) and whenever either operand is NaN"""
+    s1, s2 = np.asarray(s1, float), np.asarray(s2, float)
+    return np.where(s1 > s2, s1, s2)
+
+
+def min_(s1, s2):
+    """(s1 < s2) ? s1 : s2, the reference's min (label.H:285-297)"""
+    s1, s2 = np.asarray(s1, float), np.asarray(s2, float)
+    return np.where(s1 < s2, s1, s2)
+
+
 def _cmptAv(ic):            # VectorSpaceI.H:428-447: ((x + y) + z)/3; a scalar is its own average
     if ic.shape[1] == 1:
         return ic[:, 0].copy()

@@ -51,12 +51,12 @@ class KEpsilon:
 
     def bound(self, which, lowerBound):
         vsf, vb = getattr(self, which), getattr(self, which + "B" if which == "k" else "epsB")
-        mx, mxb = np.maximum(vsf, lowerBound), np.maximum(vb, lowerBound)
+        mx, mxb = fo.max_(vsf, lowerBound), fo.max_(vb, lowerBound)
         face = np.asarray(self.orc.interpolate_linear(self.addr, self.w, mx, 1))
         num = np.asarray(self.orc.surface_integrate(self.addr, self.magSf * face, self.bfc, self.bMagSf * mxb, self.V, 1, False, 1))
         den = np.asarray(self.orc.surface_integrate(self.addr, self.magSf, self.bfc, self.bMagSf, self.V, 1, False, 1))
         av = num / den
-        new = np.maximum(np.maximum(vsf, av * np.where(-vsf >= 0, 1.0, 0.0)), lowerBound)
+        new = fo.max_(fo.max_(vsf, av * np.where(-vsf >= 0, 1.0, 0.0)), lowerBound)
         setattr(self, which, new)
         setattr(self, "kB" if which == "k" else "epsB", mxb)
 

@@ -142,14 +142,14 @@ class Cavity:
             HbyA = rAU[:, None] * UEqn.H()
             # phiHbyA = (interpolate(HbyA) & Sf) + interpolate(rAU)*ddtCorr(U, phi)
             phiCorr = phi0 - self._dot(self.Sf, self.interpolate(U0))             # EulerDdtScheme.C:536-539
-            coeff = 1.0 - np.minimum(np.abs(phiCorr) / (np.abs(phi0) + SMALL), 1.0)   # ddtScheme.C:139-152
+            coeff = 1.0 - fo.min_(np.abs(phiCorr) / (np.abs(phi0) + SMALL), 1.0)      # ddtScheme.C:139-152
             ddtCorr = (coeff * rDeltaT) * phiCorr
             rAUf = self.interpolate(rAU)
             phiHbyA = self.flux_of(HbyA) + rAUf * ddtCorr
             bphiHbyA = self._dot(self.Ub, self.bSf)        # fixedValue: HbyA_b = U_b, coupling coefficient 0 (:156-162)
             # the same expression on the processor faces (their coupling coefficient is not zeroed)
             cphiCorr = cphi0 - self._dot(self.cSf, self.interpolate_coupled(U0))
-            ccoeff = 1.0 - np.minimum(np.abs(cphiCorr) / (np.abs(cphi0) + SMALL), 1.0)
+            ccoeff = 1.0 - fo.min_(np.abs(cphiCorr) / (np.abs(cphi0) + SMALL), 1.0)
             crAUf = self.interpolate_coupled(rAU)
             cphiHbyA = self._dot(self.interpolate_coupled(HbyA), self.cSf) + crAUf * ((ccoeff * rDeltaT) * cphiCorr)
             # adjustPhi: closed domain, the boundary flux is U_b & Sf_b = 0: nothing to adjust (adjustPhi.C)

@@ -13,6 +13,12 @@ enum { UN_NEG = 0, UN_MAG = 1, UN_S_MUL = 2, UN_S_RDIV = 3, UN_S_ADD = 4, UN_S_R
        UN_S_SUB = 8, UN_S_DIV = 9, UN_COPY = 10, UN_POS = 11 };
 enum { LIM_UPWIND = 0, LIM_LINEAR = 1, LIM_LIMITED_LINEAR = 2, LIM_VANLEER = 3, LIM_MINMOD = 4 };
 
+// max / min as the reference defines them for scalars (label.H:285-297, instantiated for doubles by doubleFloat.H:69-86):
+// the second operand on a tie (max(+0, -0) is -0) and whenever either operand is NaN, where fmax / fmin would return the
+// other operand
+__device__ __forceinline__ double ref_max(double s1, double s2) { return (s1 > s2) ? s1 : s2; }
+__device__ __forceinline__ double ref_min(double s1, double s2) { return (s1 < s2) ? s1 : s2; }
+
 __device__ __forceinline__ double bin(int op, double a, double b)
 {
     switch (op) {
@@ -20,8 +26,8 @@ __device__ __forceinline__ double bin(int op, double a, double b)
     case OP_SUB: return __dsub_rn(a, b);
     case OP_MUL: return __dmul_rn(a, b);
     case OP_DIV: return __ddiv_rn(a, b);
-    case OP_MIN: return fmin(a, b);
-    default: return fmax(a, b);
+    case OP_MIN: return ref_min(a, b);
+    default: return ref_max(a, b);
     }
 }
 
@@ -49,8 +55,8 @@ __global__ void unary_kernel(long long n, int op, double s, const double *a, dou
     case UN_S_RDIV: r = __ddiv_rn(s, x); break;
     case UN_S_ADD: r = __dadd_rn(x, s); break;
     case UN_S_RSUB: r = __dsub_rn(s, x); break;
-    case UN_S_MIN: r = fmin(x, s); break;
-    case UN_S_MAX: r = fmax(x, s); break;
+    case UN_S_MIN: r = ref_min(x, s); break;
+    case UN_S_MAX: r = ref_max(x, s); break;
     case UN_S_SUB: r = __dsub_rn(x, s); break;
     case UN_S_DIV: r = __ddiv_rn(x, s); break;
     case UN_POS: r = x >= 0 ? 1.0 : 0.0; break; // pos(), Scalar.H:119-122

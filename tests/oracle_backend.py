@@ -212,19 +212,19 @@ class FieldOps:
         return self._t(s - _np(a))
 
     def smin(self, a, s):
-        return self._t(np.minimum(_np(a), s))
+        return self._t(fo.min_(_np(a), s))
 
     def sdiv(self, a, s):
         return self._t(_np(a) / s)
 
     def smax(self, a, s):
-        return self._t(np.maximum(_np(a), s))
+        return self._t(fo.max_(_np(a), s))
 
     def pos(self, a):
         return self._t(np.where(_np(a) >= 0, 1.0, 0.0))
 
     def bmax(self, a, b):
-        return self._t(np.maximum(_np(a), _np(b)))
+        return self._t(fo.max_(_np(a), _np(b)))
 
     def symm_magsqr(self, T):
         from oracle import kepsilon_oracle as ko

@@ -20,6 +20,7 @@ import pytest
 
 import hygiene_cases as hc
 import polymesh_cases as pc
+from oracle import fvm_oracle as fo
 from test_gpu_engine_streams import environ
 
 pytestmark = pytest.mark.gpu
@@ -538,12 +539,12 @@ def field_inputs(n, seed=9):
 
 def binary_reference(op, A, B, nca, ncb):
     a, b = A.reshape(-1, nca), B.reshape(-1, ncb)
-    return np.ravel([np.add, np.subtract, np.multiply, np.divide, np.fmin, np.fmax][op](a, b))
+    return np.ravel([np.add, np.subtract, np.multiply, np.divide, fo.min_, fo.max_][op](a, b))
 
 
 def unary_reference(op, a, s):
     with np.errstate(divide="ignore"):
-        return [-a, np.abs(a), s * a, s / a, a + s, s - a, np.fmin(a, s), np.fmax(a, s), a - s, a / s, a.copy(),
+        return [-a, np.abs(a), s * a, s / a, a + s, s - a, fo.min_(a, s), fo.max_(a, s), a - s, a / s, a.copy(),
                 np.where(a >= 0, 1.0, 0.0)][op]
 
 
