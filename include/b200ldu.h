@@ -283,10 +283,41 @@ int b200ldu_fvm_relax(b200ldu_matrix *m, int nComp, double alpha, const double *
                       const double *internalCoeffs_d, double *diag_d, double *source_d);
 int b200ldu_fvm_set_reference(b200ldu_matrix *m, int celli, int nComp, const double *value_h, double *diag_d,
                               double *source_d);
+/* fvMatrix<scalar>::setValues(cells, values) (FV/fvMatrices/fvMatrix/fvMatrix.C:940-950 -> setValuesFromList :456-657, functors
+ * :350-450), in place on caller-order arrays, with the boundary faces of b200ldu_fv_boundary_set; single domain only (an
+ * addressing with coupled patches is B200LDU_EINVAL).  As the reference's device code writes it, which differs from stock
+ * OpenFOAM (DESIGN.md section 2):
+ *   psi[cells] = values; source[cells] = values*diag[cells];
+ *   every UNSET cell subtracts, owner faces first, then neighbour faces in losort order, lower[f]*value[nei] where the neighbour
+ *   is set and upper[f]*value[own] where the owner is set -- the other row's coefficient -- and keeps those couplings;
+ *   upper[f] = 0 where the owner is set, lower[f] = 0 where the neighbour is set;
+ *   internalCoeffs = boundaryCoeffs = 0 on the boundary faces of set cells.
+ * The reference asks a symmetric matrix for its non-const lower(), which makes it asymmetric with a copy of upper
+ * (lduMatrix.C:221-238): lower_d is therefore required -- a copy of upper for a symmetric matrix -- and the result is asymmetric.
+ * diag is read, not changed.  A cell listed twice must carry equal values: the reference scatters them in no defined order. */
+int b200ldu_fvm_set_values(b200ldu_matrix *m, int nSet, const int *cells_d, const double *values_d, double *psi_d,
+                           const double *diag_d, double *upper_d, double *lower_d, double *source_d, double *internalCoeffs_d,
+                           double *boundaryCoeffs_d);
 int b200ldu_fvm_solve(b200ldu_matrix *m, int nComp, const char *solver, const char *precondOrSmoother,
                       const b200ldu_controls *controls, b200ldu_gamg *gamg, double *psi_d, const double *source_d,
                       const double *internalCoeffs_d, const double *boundaryCoeffs_d, const double *pnf_d,
                       b200ldu_perf *perf);
+
+/* ---- k-epsilon wall functions (csrc/wallfn.cu; single domain, boundary faces of b200ldu_fv_boundary_set) ----
+ * b200ldu_wallfn_nutk: nutkWallFunction::calcNut (WF/nutWallFunctions/nutkWallFunction/nutkWallFunctionFvPatchScalarField.C:60-130,
+ * WF/ = src/TurbulenceModels/turbulenceModels/RAS/derivedFvPatchFields/wallFunctions/) on the nW boundary faces faces_d[]:
+ * yPlus = Cmu25*y*sqrt(k[cell])/nuw, nutB[f] = nuw*(yPlus*kappa/log(E*yPlus) - 1) if yPlus > yPlusLam, else 0.  y_d, nutB_d:
+ * [nBFaces]; yPlusLam (nutWallFunctionFvPatchScalarField.C:154-168) and Cmu25 = sqrt(sqrt(Cmu)) come from the host.
+ * b200ldu_wallfn_epsilon: epsilonWallFunction::updateCoeffs over all epsilon-wall patches (epsilonWallFunctionFvPatchScalarField.C
+ * :231-262, :334-400, :540-590): per wall cell epsilon0 = sum w*Cmu75*pow(k, 1.5)/(kappa*y) and G0 = sum w*(nutB + nu)*
+ * mag(deltaCoeffs*(Ub - U[cell]))*Cmu25*sqrt(k)/(kappa*y) over its wall faces (patch order, faces ascending, from 0), then
+ * G = G0, epsilon = epsilon0 in the cell and epsB = epsilon0 on its wall faces, in place.  cornerWeights_d [nBFaces]: 1/(the
+ * number of epsilon-wall faces of the face's cell), 0 on faces of other patches; U_d [nCells*3], Ub_d [nBFaces*3]. */
+int b200ldu_wallfn_nutk(b200ldu_addr *a, int nW, const int *faces_d, const double *y_d, const double *k_d, double nuw,
+                        double yPlusLam, double Cmu25, double kappa, double E, double *nutB_d);
+int b200ldu_wallfn_epsilon(b200ldu_addr *a, const double *cornerWeights_d, const double *y_d, const double *k_d, const double *U_d,
+                           const double *Ub_d, const double *bDelta_d, const double *nutB_d, double nu, double Cmu25, double Cmu75,
+                           double kappa, double *G_d, double *epsilon_d, double *epsB_d);
 
 /* ---- element-wise field operators between the kernels (SURVEY.md section 8(f) rank 2; the gpuField operator set of
  * src/OpenFOAM/fields/Fields/gpuField/gpuFieldFunctionsM.C:200-330): one rounding per element and operator, so a

@@ -69,6 +69,7 @@ EXPORTS = [
     "b200ldu_fvm_flux", "b200ldu_fvm_residual", "b200ldu_fvm_relax", "b200ldu_fvm_set_reference",
     "b200ldu_fvm_solve", "b200ldu_fv_patch_neighbour_field",
     "b200ldu_mules_limiter", "b200ldu_mules_limiter_corr", "b200ldu_ldu_row_sum", "b200ldu_ldu_add_assign", "b200ldu_ldu_scale", "b200ldu_fv_sngrad", "b200ldu_fv_limiter", "b200ldu_fv_limited_weights", "b200ldu_field_binary", "b200ldu_field_unary", "b200ldu_field_dot3", "b200ldu_field_symm_magsqr", "b200ldu_field_gather",
+    "b200ldu_fvm_set_values", "b200ldu_wallfn_nutk", "b200ldu_wallfn_epsilon",
 ]
 
 _lib = None
@@ -163,6 +164,9 @@ def lib():
     L.b200ldu_field_dot3.argtypes = [vp, C.c_longlong, vp, vp, vp]
     L.b200ldu_field_symm_magsqr.argtypes = [vp, C.c_longlong, vp, vp]
     L.b200ldu_field_gather.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp]
+    L.b200ldu_fvm_set_values.argtypes = [vp, C.c_int] + [vp] * 9
+    L.b200ldu_wallfn_nutk.argtypes = [vp, C.c_int, vp, vp, vp] + [C.c_double] * 5 + [vp]
+    L.b200ldu_wallfn_epsilon.argtypes = [vp] + [vp] * 7 + [C.c_double] * 4 + [vp] * 3
     L.b200ldu_fvm_solve.argtypes = [vp, C.c_int, C.c_char_p, C.c_char_p, C.POINTER(Controls), vp, vp, vp, vp, vp, vp,
                                     C.POINTER(Perf)]
     _lib = L
@@ -443,6 +447,14 @@ class FvMatrix:
         v = np.ascontiguousarray(np.atleast_1d(np.asarray(value, np.float64)))
         check(lib().b200ldu_fvm_set_reference(self.m.h, int(celli), self.nc, _hp(v), _dp(self.diag), _dp(self.source)))
 
+    def setValues(self, cells, values, upper, lower):
+        """fvMatrix::setValues (scalar, single domain), in place on psi, source, upper, lower, internalCoeffs and
+        boundaryCoeffs; `lower` is required (a copy of upper for a symmetric matrix: the result is asymmetric, see
+        b200ldu.h).  cells: int32 device tensor, a cell listed twice with equal values.  The LduMatrix has to be set()
+        again before it is used."""
+        check(lib().b200ldu_fvm_set_values(self.m.h, cells.numel(), _dp(cells), _dp(values), _dp(self.psi), _dp(self.diag),
+                                           _dp(upper), _dp(lower), _dp(self.source), _dp(self.ic), _dp(self.bc)))
+
     def solve(self, solver, pre, gamg=None, pnf=None, **ctl):
         """solveSegregated: psi updated in place; returns the list of Perf, one per component"""
         c = controls(**ctl)
@@ -572,6 +584,18 @@ class FieldOps:
 def _newlike(t, n):
     import torch
     return torch.empty(n, dtype=torch.float64, device=t.device)
+
+
+def wallfn_nutk(addr, faces, y, k, nuw, yPlusLam, Cmu25, nutB, kappa=0.41, E=9.8):
+    """nutkWallFunction::calcNut into nutB at the boundary faces `faces` (int32 device tensor), in place"""
+    check(lib().b200ldu_wallfn_nutk(addr.h, faces.numel(), _dp(faces), _dp(y), _dp(k), float(nuw), float(yPlusLam), float(Cmu25),
+                                    float(kappa), float(E), _dp(nutB)))
+
+
+def wallfn_epsilon(addr, cornerWeights, y, k, U, Ub, bDelta, nutB, nu, Cmu25, Cmu75, G, epsilon, epsB, kappa=0.41):
+    """epsilonWallFunction::updateCoeffs of all epsilon-wall patches: G, epsilon and epsB in place (b200ldu.h)"""
+    check(lib().b200ldu_wallfn_epsilon(addr.h, _dp(cornerWeights), _dp(y), _dp(k), _dp(U), _dp(Ub), _dp(bDelta), _dp(nutB),
+                                       float(nu), float(Cmu25), float(Cmu75), float(kappa), _dp(G), _dp(epsilon), _dp(epsB)))
 
 
 def fv_convection_fill(addr, weights, phi):

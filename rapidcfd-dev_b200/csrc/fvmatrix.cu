@@ -1,7 +1,7 @@
 // fvmatrix.cu -- the fvMatrix glue around the linear solvers (SURVEY.md section 8, row a17), caller-order
 // fields.  Reference (FV/ = src/finiteVolume/): addBoundaryDiag / addCmptAvBoundaryDiag / addBoundarySource
 // FV/fvMatrices/fvMatrix/fvMatrix.C:209-348; setReference :965-983; relax :1088-1345; D / A :1375-1455;
-// H :1458-1508 (scalar: fvScalarMatrix.C:252-283); flux :1591-1660; residual fvScalarMatrix.C:195-240;
+// setValues :456-657; H :1458-1508 (scalar: fvScalarMatrix.C:252-283); flux :1591-1660; residual fvScalarMatrix.C:195-240;
 // solveSegregated fvScalarMatrix.C:142-192 (scalar), fvMatrixSolve.C:104-226 (component loop).
 //
 // Boundary model (same as oracle/fvm_oracle.py): the non-coupled boundary faces of all patches are the flat list
@@ -177,6 +177,38 @@ extern "C" int b200ldu_fvm_set_reference(b200ldu_matrix *m, int celli, int nComp
     CUDA_TRY(cudaSetDevice(a->ctx->device));
     return launch(a->ctx, set_reference_kernel, 1, 1, celli, nComp, value_h[0], nComp > 1 ? value_h[1] : 0.0,
                   nComp > 2 ? value_h[2] : 0.0, diag_d, source_d);
+}
+
+// setValues (fvMatrix.C:940-950 -> setValuesFromList :456-657) as the reference's device code writes it; see b200ldu.h
+extern "C" int b200ldu_fvm_set_values(b200ldu_matrix *m, int nSet, const int *cells_d, const double *values_d, double *psi_d,
+                                      const double *diag_d, double *upper_d, double *lower_d, double *source_d,
+                                      double *internalCoeffs_d, double *boundaryCoeffs_d)
+{
+    if (!m || nSet < 0 || (nSet && (!cells_d || !values_d)) || !psi_d || !diag_d || !source_d) return B200LDU_EINVAL;
+    b200ldu_addr *a = m->a;
+    if (a->nPatches) {
+        b200_set_error("fvm_set_values: single domain only (the addressing has %d coupled patches)", a->nPatches);
+        return B200LDU_EINVAL;
+    }
+    if (a->nFaces && (!upper_d || !lower_d)) {
+        b200_set_error("fvm_set_values: upper and lower required (a symmetric matrix leaves asymmetric: pass a copy of upper as "
+                       "lower, as lduMatrix::lower() makes one)");
+        return B200LDU_EINVAL;
+    }
+    TRY(need_boundary(a, internalCoeffs_d, "fvm_set_values"));
+    TRY(need_boundary(a, boundaryCoeffs_d, "fvm_set_values"));
+    CUDA_TRY(cudaSetDevice(a->ctx->device));
+    b200ldu_ctx *ctx = a->ctx;
+    const int n = a->nCells;
+    int *mask = nullptr;
+    TRY(a->mem.slot(ADDR_FVM_SET_MASK, mask, (size_t)n));
+    TRY(launch(ctx, set_values_clear_mask_kernel, n, 256, n, mask));
+    TRY(launch(ctx, set_values_scatter_kernel, nSet, 256, nSet, cells_d, values_d, diag_d, mask, psi_d, source_d));
+    TRY(launch(ctx, set_values_source_kernel, n, 128, n, a->d_ownerStart, a->d_u, a->d_losortStart, a->d_losort, a->d_l, upper_d,
+               lower_d, mask, psi_d, source_d));
+    TRY(launch(ctx, set_values_faces_kernel, a->nFaces, 256, a->nFaces, a->d_l, a->d_u, mask, upper_d, lower_d));
+    return launch(ctx, set_values_boundary_kernel, a->nBFaces, 256, a->nBFaces, a->d_bFaceCells, mask, internalCoeffs_d,
+                  boundaryCoeffs_d);
 }
 
 // solveSegregated: fold the boundary into diagonal and source, solve, put the diagonal back.

@@ -320,6 +320,69 @@ __global__ void set_reference_kernel(int cell, int nc, double v0, double v1, dou
         source[(size_t)cell * nc + k] = __dadd_rn(source[(size_t)cell * nc + k], __dmul_rn(d, v[k]));
     diag[cell] = __dmul_rn(2.0, d);
 }
+
+// setValues (fvMatrix.C:456-657, functors :350-450) over caller-order arrays: clear the mask, scatter, source, faces, boundary.  mask[c] != 0 marks a set cell;
+// psi holds the set values by the time the source pass reads them (the reference's cellValuesTmp equals psi there).
+__global__ void set_values_clear_mask_kernel(int nCells, int *mask)
+{
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c < nCells) mask[c] = 0;
+}
+
+// psi[cells] = values, source[cells] = values*diag[cells] (:471-497); a cell listed twice carries equal values
+__global__ void set_values_scatter_kernel(int nSet, const int *__restrict__ cells, const double *__restrict__ values,
+                                          const double *__restrict__ diag, int *mask, double *psi, double *source)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= nSet) return;
+    const int c = cells[i];
+    const double v = values[i];
+    psi[c] = v;
+    source[c] = __dmul_rn(v, diag[c]);
+    mask[c] = 1;
+}
+
+// fvMatrixSetValuesSourceFunctor: an unset cell subtracts lower*psi[nei] on its owner faces whose neighbour is set, then
+// upper*psi[own] on its neighbour faces (losort order) whose owner is set -- the other row's coefficient, as the reference has it
+__global__ void set_values_source_kernel(int nCells, const int *__restrict__ ownerStart, const int *__restrict__ u,
+                                         const int *__restrict__ losortStart, const int *__restrict__ losort,
+                                         const int *__restrict__ l, const double *__restrict__ upper,
+                                         const double *__restrict__ lower, const int *__restrict__ mask,
+                                         const double *__restrict__ psi, double *__restrict__ source)
+{
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= nCells || mask[c]) return;
+    double out = source[c];
+    for (int f = ownerStart[c]; f < ownerStart[c + 1]; f++) {
+        const int n = u[f];
+        if (mask[n]) out = __dsub_rn(out, __dmul_rn(lower[f], psi[n]));
+    }
+    for (int q = losortStart[c]; q < losortStart[c + 1]; q++) {
+        const int f = losort[q], o = l[f];
+        if (mask[o]) out = __dsub_rn(out, __dmul_rn(upper[f], psi[o]));
+    }
+    source[c] = out;
+}
+
+// upper = 0 where the owner is set, lower = 0 where the neighbour is set (:600-622; the matrix is asymmetric by then)
+__global__ void set_values_faces_kernel(int nFaces, const int *__restrict__ l, const int *__restrict__ u,
+                                        const int *__restrict__ mask, double *__restrict__ upper, double *__restrict__ lower)
+{
+    const int f = blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= nFaces) return;
+    if (mask[l[f]]) upper[f] = 0.0;
+    if (mask[u[f]]) lower[f] = 0.0;
+}
+
+// internalCoeffs = boundaryCoeffs = 0 on the boundary faces of set cells (:624-655)
+__global__ void set_values_boundary_kernel(int nB, const int *__restrict__ faceCells, const int *__restrict__ mask,
+                                           double *__restrict__ ic, double *__restrict__ bc)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= nB || !mask[faceCells[i]]) return;
+    ic[i] = 0.0;
+    bc[i] = 0.0;
+}
 } // namespace
 } // namespace fvmk
 #endif

@@ -277,6 +277,7 @@ enum AddrSlot {
     // fvMatrix glue (fvmatrix.cu): cell fields of fvm_solve / fvm_residual, and the patch-face send buffer of
     // fv_patch_neighbour_field, which shares its slot with the component psi of fvm_solve
     ADDR_FVM_DIAG, ADDR_FVM_SOURCE, ADDR_FVM_CMPT_SOURCE, ADDR_FVM_CMPT_PSI,
+    ADDR_FVM_SET_MASK, // fvm_set_values: the set-cell mask
     ADDR_MULES, // MULES limiter: six cell fields and the received limiters (mules.cu)
 };
 

@@ -687,6 +687,63 @@ class PolyMesh:
         delta = 1.0 / np.linalg.norm(C[nei] - C[own], axis=1)
         return dict(C=C, V=V, Cf=Cf, Sf=Sf, magSf=np.linalg.norm(Sf, axis=1), weights=w, deltaCoeffs=delta)
 
+    def near_wall_dist(self, wallPatches=None):
+        """nearWallDist::correct (finiteVolume/fvMesh/wallDist/nearWallDist.C:40-100): for every face of a wall patch, the
+        distance from its cell centre to the nearest of the face and its point neighbours on the same patch
+        (cellDistFuncs::getPointNeighbours / smallestDist, meshTools/cellDist/cellDistFuncs.C:82-170), each face taken as the
+        triangle fan about its point average (face::nearestPoint).  Returns y of every boundary face in patch order, 0 on the
+        other patches.  wallPatches: names of the wall patches (default: the patches of type wall).  Once per mesh."""
+        C, _ = self.cell_centres_and_volumes()
+        nI = self.nInternalFaces
+        y = np.zeros(len(self.owner) - nI)
+        for p in self.patches:
+            if not (p.name in wallPatches if wallPatches is not None else p.type == "wall"):
+                continue
+            faces = [self.faceLabels[self.faceOffsets[f]:self.faceOffsets[f + 1]] for f in range(p.startFace, p.startFace + p.nFaces)]
+            pointFaces = {}
+            for i, f in enumerate(faces):
+                for q in f:
+                    pointFaces.setdefault(int(q), []).append(i)
+            for i, f in enumerate(faces):
+                nbrs = {i}.union(*(pointFaces[int(q)] for q in f))
+                c = C[self.owner[p.startFace + i]]
+                y[p.startFace - nI + i] = min(_face_distance(c, self.points[faces[j]]) for j in nbrs)
+        return y
+
+
+def _triangle_distance(p, a, b, c):
+    """distance from p to the closest point of triangle abc (Ericson, Real-Time Collision Detection 5.1.5)"""
+    ab, ac, ap = b - a, c - a, p - a
+    d1, d2 = ab @ ap, ac @ ap
+    if d1 <= 0 and d2 <= 0:
+        return float(np.linalg.norm(ap))
+    bp = p - b
+    d3, d4 = ab @ bp, ac @ bp
+    if d3 >= 0 and d4 <= d3:
+        return float(np.linalg.norm(bp))
+    vc = d1 * d4 - d3 * d2
+    if vc <= 0 and d1 >= 0 and d3 <= 0:
+        return float(np.linalg.norm(p - (a + ab * (d1 / (d1 - d3)))))
+    cp = p - c
+    d5, d6 = ab @ cp, ac @ cp
+    if d6 >= 0 and d5 <= d6:
+        return float(np.linalg.norm(cp))
+    vb = d5 * d2 - d1 * d6
+    if vb <= 0 and d2 >= 0 and d6 <= 0:
+        return float(np.linalg.norm(p - (a + ac * (d2 / (d2 - d6)))))
+    va = d3 * d6 - d5 * d4
+    if va <= 0 and (d4 - d3) >= 0 and (d5 - d6) >= 0:
+        return float(np.linalg.norm(p - (b + (c - b) * ((d4 - d3) / ((d4 - d3) + (d5 - d6))))))
+    den = 1.0 / (va + vb + vc)
+    return float(np.linalg.norm(p - (a + ab * (vb * den) + ac * (vc * den))))
+
+
+def _face_distance(p, pts):
+    """distance from p to a face given by its points: the triangle itself, or the fan of triangles about the point average"""
+    if len(pts) == 3:
+        return _triangle_distance(p, pts[0], pts[1], pts[2])
+    ctr = pts.mean(axis=0)
+    return min(_triangle_distance(p, pts[k], pts[(k + 1) % len(pts)], ctr) for k in range(len(pts)))
 
 def read_boundary(path):
     raw = _read_bytes(path)
