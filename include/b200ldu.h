@@ -204,6 +204,30 @@ int b200ldu_gamg_nlevels(const b200ldu_gamg *g);
 int b200ldu_gamg_level_size(const b200ldu_gamg *g, int lev, int *nCells, int *nFaces);
 /* HOST copies of the level maps (parity tests): restrictAddressing of level lev */
 int b200ldu_gamg_restrict_addr(const b200ldu_gamg *g, int lev, int *out_h);
+/* HOST copies of what coarse level lev (as restrict_addr) holds, for parity tests.  Returns the element count and
+ * copies at most cap elements to out_h (which may be NULL), or B200LDU_EINVAL for a bad lev / what.  Waits for the
+ * context stream; changes nothing a later solve sees.
+ *   OWNER, NEIGHBOUR   int[nCoarseFaces]  coarse addressing, caller order
+ *   FACE_RESTRICT      int[nFineFaces]    fine face -> coarse face, or -(coarse cell + 1) where it collapses into one
+ *   FACE_FLIP          int[nFineFaces]    1 where the coarse face runs against the fine one (0 for collapsed faces)
+ *   DIAG, UPPER, LOWER double             the last solve's coarse coefficients, caller order; LOWER has 0 elements
+ *                                         when that matrix was symmetric
+ *   BOU, INT           double             its restricted interface coefficients, coarse patch-face order
+ *   PERM               int[nCoarse]       the level's banded row of every coarse cell
+ *   INV                double[n * N]      coarsest level only: this rank's rows of the inverse of the coarsest
+ *                                         matrix as the solve uploaded them -- banded rows, global banded columns
+ *   INV_DIMS           int[3]             coarsest level only: {N, this rank's first row, n}
+ * The addressing codes (OWNER ... FACE_FLIP) also serve a host-only hierarchy; coefficients need a solve with
+ * this handle first, INV and INV_DIMS a solve with directSolveCoarsest. */
+enum {
+    B200LDU_GAMG_OWNER, B200LDU_GAMG_NEIGHBOUR, B200LDU_GAMG_FACE_RESTRICT, B200LDU_GAMG_FACE_FLIP,
+    B200LDU_GAMG_DIAG, B200LDU_GAMG_UPPER, B200LDU_GAMG_LOWER, B200LDU_GAMG_BOU, B200LDU_GAMG_INT,
+    B200LDU_GAMG_PERM, B200LDU_GAMG_INV, B200LDU_GAMG_INV_DIMS
+};
+long long b200ldu_gamg_debug_get(const b200ldu_gamg *g, int lev, int what, void *out_h, long long cap);
+/* The host inverse a GAMG solve uploads for its coarsest level (partial-pivot Gauss-Jordan), on its own: inv_h = A_h^-1,
+ * both HOST row-major N x N.  Returns the number of row swaps, or B200LDU_EINVAL for a singular A_h.  No GPU. */
+int b200ldu_gamg_debug_invert(int N, const double *A_h, double *inv_h);
 
 /* ---- finiteVolume face-sum loops (caller-order device fields) ----
  * nComp = 1 or 3, AoS.  Boundary faces of all patches concatenated in patch order.

@@ -176,6 +176,18 @@ const int *orc_gamg_patch_face_restrict(const orc_gamg *g, int lev); /* fine pat
 /* GAMGInterface::agglomerateCoeffs over all patches of level lev (GAMGInterface.C:120-172): coarse[cpf] = sum of
  * the fine coefficients mapped to it, in ascending fine patch-face order */
 void orc_gamg_agglomerate_patch_coeffs(const orc_gamg *g, int lev, const double *fine, double *coarse);
+/* coarse level lev's matrix for the finest matrix m as orc_gamg_solve builds it: diag[nCells], upper/lower[nFaces]
+ * (lower written for an asymmetric m only; may be NULL), restricted interface coefficients bou/intc[npatchfaces]
+ * (may be NULL) */
+void orc_gamg_coarse_matrix(const orc_matrix *m, const orc_gamg *g, int lev, double *diag, double *upper,
+                            double *lower, double *bou, double *intc);
+/* Opt-in coarsest solve of a given inverse instead of the LU (invRows NULL: back to the LU).  invRows holds this
+ * rank's rows of the inverse of the global coarsest matrix, row-major nCells x N, indexed by banded row and by global
+ * banded column (rank offset + banded row); perm gives every coarsest cell's banded row.  The correction is
+ * x[c] = sum_j inv[perm[c]][j] * b[j], one fused multiply-add per term in ascending j. */
+void orc_gamg_set_coarsest_inverse(orc_gamg *g, const double *invRows, const int *perm, int N);
+/* descending != 0: the scaling's two sums run from the last cell down (calibrates tolerances for other orders) */
+void orc_gamg_set_scale_order(orc_gamg *g, int descending);
 
 /* ---- finite-volume face-sum loops (Appendix A.11) ---- */
 void orc_sngrad(const orc_addr *a, int nComp, const double *deltaCoeffs, const double *vf, double *out);

@@ -111,6 +111,9 @@ def lib():
         L.orc_gamg_patch_face_restrict.restype = c_ip
         L.orc_gamg_patch_face_restrict.argtypes = [C.c_void_p, C.c_int]
         L.orc_gamg_agglomerate_patch_coeffs.argtypes = [C.c_void_p, C.c_int, c_dp, c_dp]
+        L.orc_gamg_coarse_matrix.argtypes = [C.c_void_p, C.c_void_p, C.c_int, c_dp, c_dp, c_dp, c_dp, c_dp]
+        L.orc_gamg_set_coarsest_inverse.argtypes = [C.c_void_p, c_dp, c_ip, C.c_int]
+        L.orc_gamg_set_scale_order.argtypes = [C.c_void_p, C.c_int]
         L.orc_addr_npatches.argtypes = [C.c_void_p]
         for nm in ("orc_addr_patch_start", "orc_addr_face_cells"):
             getattr(L, nm).restype = c_ip
@@ -419,6 +422,27 @@ class Gamg:
         out = np.zeros(max(self.npatchfaces(lev), 1))
         lib().orc_gamg_agglomerate_patch_coeffs(self.h, lev, _d(f64(fine)), _d(out))
         return out[: self.npatchfaces(lev)]
+
+    def coarse_matrix(self, matrix, lev):
+        """dict(diag, upper, lower, bou, int) of coarse level lev for the finest `matrix`, as the solve builds it
+        (lower None for a symmetric matrix)"""
+        n, nf, npf = self.ncells(lev), self.nfaces(lev), self.npatchfaces(lev)
+        d, u, lo, b, i = (np.zeros(max(k, 1)) for k in (n, nf, nf, npf, npf))
+        lib().orc_gamg_coarse_matrix(matrix.h, self.h, lev, _d(d), _d(u), _d(lo), _d(b), _d(i))
+        return dict(diag=d[:n], upper=u[:nf], lower=None if matrix.lower is None else lo[:nf], bou=b[:npf], int=i[:npf])
+
+    def set_coarsest_inverse(self, inv=None, perm=None):
+        """Solve the coarsest level with the given rows of an inverse (this rank's banded rows x N global banded
+        columns) and banded permutation, one FMA chain per row as the device applies it; None: the LU again."""
+        if inv is None:
+            lib().orc_gamg_set_coarsest_inverse(self.h, None, None, 0)
+            return
+        inv = f64(inv)
+        self._inv = (inv, i32(perm))
+        lib().orc_gamg_set_coarsest_inverse(self.h, _d(inv), _i(self._inv[1]), inv.shape[1])
+
+    def set_scale_order(self, descending):
+        lib().orc_gamg_set_scale_order(self.h, int(bool(descending)))
 
     def level_addr(self, lev):
         a = Addr(self.ncells(lev), None, None, _handle=lib().orc_gamg_addr(self.h, lev))

@@ -31,6 +31,11 @@ struct orc_gamg {
     int *patchFaceRestrict[ORC_MAX_LEVELS]; /* fine patch face (flat) -> coarse patch face (flat) */
     int nFinePatchFaces[ORC_MAX_LEVELS];
     const orc_addr *finest;
+    /* opt-in coarsest solve with a given inverse (orc_gamg_set_coarsest_inverse) */
+    double *devInv; /* this rank's rows of the inverse, row-major nCoarsest x devN */
+    int *devPerm;   /* banded row of every coarsest cell */
+    int devN;
+    int scaleDescending; /* orc_gamg_set_scale_order */
 };
 
 /* pairGAMGAgglomeration::agglomerate(nCoarseCells, addr, faceWeights):
@@ -356,6 +361,8 @@ void orc_gamg_free(orc_gamg *g)
         free(g->faceFlip[i]);
         free(g->patchFaceRestrict[i]);
     }
+    free(g->devInv);
+    free(g->devPerm);
     free(g);
 }
 
@@ -454,13 +461,18 @@ static void agglomerate_matrix(const orc_gamg *g, int lev, const double *fd, con
 
 /* scale: GAMGSolverScale.C:59-171 */
 static void gamg_scale(const orc_matrix *A, double *field, double *Acf, const double *source,
-                       const orc_comm *comm)
+                       const orc_comm *comm, int descending)
 {
     int n = A->a->nCells;
     orc_amul(A, field, Acf, comm);
     double num = 0, den = 0;
-    for (int i = 0; i < n; i++) num += source[i] * field[i];
-    for (int i = 0; i < n; i++) den += Acf[i] * field[i];
+    if (descending) { /* the same two sums in the other order: a measure of what any other order may change */
+        for (int i = n - 1; i >= 0; i--) num += source[i] * field[i];
+        for (int i = n - 1; i >= 0; i--) den += Acf[i] * field[i];
+    } else {
+        for (int i = 0; i < n; i++) num += source[i] * field[i];
+        for (int i = 0; i < n; i++) den += Acf[i] * field[i];
+    }
     if (comm && comm->sum) { /* vector2D all-reduce: GAMGSolverScale.C:139-140 */
         double v[2] = {num, den};
         comm->sum(comm->ctx, v, 2);
@@ -673,6 +685,86 @@ static void lu_solve(const dense_lu *d, const double *bLocal, double *xLocal, co
     free(b);
 }
 
+void orc_gamg_set_coarsest_inverse(orc_gamg *g, const double *invRows, const int *perm, int N)
+{
+    free(g->devInv);
+    free(g->devPerm);
+    g->devInv = NULL;
+    g->devPerm = NULL;
+    g->devN = 0;
+    if (!invRows || g->nLevels == 0) return;
+    int n = g->addr[g->nLevels - 1]->nCells;
+    g->devN = N;
+    g->devInv = (double *)malloc(sizeof(double) * ((size_t)n * N + 1));
+    g->devPerm = (int *)malloc(sizeof(int) * ((size_t)n + 1));
+    memcpy(g->devInv, invRows, sizeof(double) * (size_t)n * N);
+    memcpy(g->devPerm, perm, sizeof(int) * (size_t)n);
+}
+
+void orc_gamg_set_scale_order(orc_gamg *g, int descending) { g->scaleDescending = descending; }
+
+/* x[c] = sum_j inv[perm[c]][j] * bg[j] with bg the right-hand sides of all ranks in banded order (rank offset +
+ * banded row), one fused multiply-add per term in ascending j from zero */
+static void dev_inverse_apply(const orc_gamg *g, int n, const double *b, double *x, const orc_comm *comm)
+{
+    int N = g->devN, R = (comm && comm->gather && comm->nRanks > 1) ? comm->nRanks : 1;
+    double *bg = (double *)calloc((size_t)N + 1, sizeof(double));
+    if (R > 1) {
+        double mine = n, *cnt = (double *)calloc((size_t)R, sizeof(double));
+        comm->gather(comm->ctx, &mine, 1, cnt);
+        int nMax = 0;
+        for (int r = 0; r < R; r++) nMax = (int)cnt[r] > nMax ? (int)cnt[r] : nMax;
+        double *bb = (double *)calloc((size_t)nMax + 1, sizeof(double));
+        double *all = (double *)calloc((size_t)R * nMax + 1, sizeof(double));
+        for (int c = 0; c < n; c++) bb[g->devPerm[c]] = b[c];
+        comm->gather(comm->ctx, bb, nMax, all);
+        for (int r = 0, o = 0; r < R; o += (int)cnt[r], r++)
+            memcpy(bg + o, all + (size_t)r * nMax, sizeof(double) * (size_t)cnt[r]);
+        free(cnt);
+        free(bb);
+        free(all);
+    } else
+        for (int c = 0; c < n; c++) bg[g->devPerm[c]] = b[c];
+    for (int c = 0; c < n; c++) {
+        const double *row = g->devInv + (size_t)g->devPerm[c] * N;
+        double s = 0.0;
+        for (int j = 0; j < N; j++) s = fma(row[j], bg[j], s);
+        x[c] = s;
+    }
+    free(bg);
+}
+
+/* the coarse matrix of level lev for the finest matrix m, as the solve builds it */
+void orc_gamg_coarse_matrix(const orc_matrix *m, const orc_gamg *g, int lev, double *diag, double *upper,
+                            double *lower, double *bou, double *intc)
+{
+    lev_matrix *lm = (lev_matrix *)calloc((size_t)lev + 1, sizeof(lev_matrix));
+    for (int k = 0; k <= lev; k++) {
+        const double *fd = k ? lm[k - 1].diag : m->diag;
+        const double *fu = k ? lm[k - 1].upper : m->upper;
+        const double *fl = k ? lm[k - 1].lower : (m->symmetric ? NULL : m->lower);
+        const double *fb = k ? lm[k - 1].bou : m->bou;
+        const double *fi = k ? lm[k - 1].intc : m->intc;
+        agglomerate_matrix(g, k, fd, fu, fl, fb, fi, &lm[k]);
+    }
+    const lev_matrix *L = &lm[lev];
+    int nCP = orc_gamg_npatchfaces(g, lev);
+    memcpy(diag, L->diag, sizeof(double) * (size_t)L->n);
+    memcpy(upper, L->upper, sizeof(double) * (size_t)L->nf);
+    if (lower && L->lower) memcpy(lower, L->lower, sizeof(double) * (size_t)L->nf);
+    if (bou) memcpy(bou, L->bou, sizeof(double) * (size_t)nCP);
+    if (intc) memcpy(intc, L->intc, sizeof(double) * (size_t)nCP);
+    for (int k = 0; k <= lev; k++) {
+        free(lm[k].diag);
+        free(lm[k].upper);
+        free(lm[k].lower);
+        free(lm[k].bou);
+        free(lm[k].intc);
+        orc_matrix_free(lm[k].m);
+    }
+    free(lm);
+}
+
 static int imin(int a, int b) { return a < b ? a : b; }
 
 /* GAMGSolver::solve + Vcycle: GAMGSolverSolve.C:59-474 */
@@ -701,7 +793,7 @@ int orc_gamg_solve(const orc_matrix *m, orc_gamg *g, const char *smoother, const
         agglomerate_matrix(g, lev, fd, fu, fl, fb, fi, &lm[lev]);
     }
     int coarsest = nL - 1;
-    dense_lu *lu = c->directSolveCoarsest ? lu_factor(lm[coarsest].m, comm) : NULL;
+    dense_lu *lu = c->directSolveCoarsest && !g->devInv ? lu_factor(lm[coarsest].m, comm) : NULL;
 
     double *Apsi = (double *)calloc((size_t)n, sizeof(double));
     double *finestCorr = (double *)calloc((size_t)n, sizeof(double));
@@ -741,7 +833,7 @@ int orc_gamg_solve(const orc_matrix *m, orc_gamg *g, const char *smoother, const
                                       comm);
                     double *ACf = scratch1;
                     if (scaleCorrection && lev < coarsest - 1)
-                        gamg_scale(lm[lev].m, corr[lev], ACf, src[lev], comm);
+                        gamg_scale(lm[lev].m, corr[lev], ACf, src[lev], comm, g->scaleDescending);
                     orc_amul(lm[lev].m, corr[lev], ACf, comm);
                     for (int i = 0; i < lm[lev].n; i++) src[lev][i] -= ACf[i];
                 }
@@ -749,7 +841,9 @@ int orc_gamg_solve(const orc_matrix *m, orc_gamg *g, const char *smoother, const
                                src[lev + 1]);
             }
             /* solveCoarsestLevel :552-619 */
-            if (c->directSolveCoarsest) {
+            if (c->directSolveCoarsest && g->devInv) {
+                dev_inverse_apply(g, lm[coarsest].n, src[coarsest], corr[coarsest], comm);
+            } else if (c->directSolveCoarsest) {
                 lu_solve(lu, src[coarsest], corr[coarsest], comm);
             } else {
                 orc_controls cc;
@@ -768,7 +862,7 @@ int orc_gamg_solve(const orc_matrix *m, orc_gamg *g, const char *smoother, const
                 double *ACf = scratch1;
                 if (c->interpolateCorrection) gamg_interpolate(lm[lev].m, corr[lev], ACf, comm);
                 if (scaleCorrection && (c->interpolateCorrection || lev < coarsest - 1))
-                    gamg_scale(lm[lev].m, corr[lev], ACf, src[lev], comm);
+                    gamg_scale(lm[lev].m, corr[lev], ACf, src[lev], comm, g->scaleDescending);
                 if (c->nPreSweeps)
                     for (int i = 0; i < lm[lev].n; i++) corr[lev][i] += pre[i];
                 orc_jacobi_smooth(lm[lev].m, c->omega, corr[lev], src[lev],
@@ -778,7 +872,7 @@ int orc_gamg_solve(const orc_matrix *m, orc_gamg *g, const char *smoother, const
             }
             prolong_field(g->restrictAddr[0], n, corr[0], finestCorr);
             if (c->interpolateCorrection) gamg_interpolate(m, finestCorr, Apsi, comm);
-            if (scaleCorrection) gamg_scale(m, finestCorr, Apsi, finestRes, comm);
+            if (scaleCorrection) gamg_scale(m, finestCorr, Apsi, finestRes, comm, g->scaleDescending);
             for (int i = 0; i < n; i++) psi[i] = psi[i] + finestCorr[i];
             orc_jacobi_smooth(m, c->omega, psi, source, c->nFinestSweeps, comm);
             /* ---- end Vcycle ---- */

@@ -60,7 +60,7 @@ EXPORTS = [
     "b200ldu_vec_len", "b200ldu_to_banded", "b200ldu_from_banded", "b200ldu_amul_banded",
     "b200ldu_solve", "b200ldu_solve_host", "b200ldu_launch_count", "b200ldu_ctx_device_mem", "b200ldu_bench_op",
     "b200ldu_gamg_create", "b200ldu_gamg_destroy", "b200ldu_gamg_nlevels", "b200ldu_gamg_level_size",
-    "b200ldu_gamg_restrict_addr",
+    "b200ldu_gamg_restrict_addr", "b200ldu_gamg_debug_get", "b200ldu_gamg_debug_invert",
     "b200ldu_fv_boundary_set", "b200ldu_fv_surface_integrate", "b200ldu_fv_gauss_grad",
     "b200ldu_fv_laplacian_fill", "b200ldu_fv_convection_fill", "b200ldu_fv_interpolate_linear",
     "b200ldu_fv_add_boundary_diag", "b200ldu_fv_add_boundary_source", "b200ldu_fv_grad_linear",
@@ -130,6 +130,9 @@ def lib():
     L.b200ldu_gamg_nlevels.argtypes = [vp]
     L.b200ldu_gamg_level_size.argtypes = [vp, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]
     L.b200ldu_gamg_restrict_addr.argtypes = [vp, C.c_int, vp]
+    L.b200ldu_gamg_debug_get.restype = C.c_longlong
+    L.b200ldu_gamg_debug_get.argtypes = [vp, C.c_int, C.c_int, vp, C.c_longlong]
+    L.b200ldu_gamg_debug_invert.argtypes = [C.c_int, vp, vp]
     L.b200ldu_fv_boundary_set.argtypes = [vp, C.c_int, vp]
     L.b200ldu_fv_surface_integrate.argtypes = [vp, C.c_int, vp, vp, vp, vp, C.c_int, C.c_int]
     L.b200ldu_fv_gauss_grad.argtypes = [vp, C.c_int, vp, vp, vp, vp, vp, vp]
@@ -489,6 +492,42 @@ class GamgAgglomeration:
         out = np.zeros(n, dtype=np.int32)
         check(lib().b200ldu_gamg_restrict_addr(self.h, lev, _hp(out)))
         return out
+
+    # b200ldu_gamg_debug_get's codes, in order, with the element type of each
+    DEBUG = [("owner", np.int32), ("neighbour", np.int32), ("faceRestrict", np.int32), ("faceFlip", np.int32),
+             ("diag", np.float64), ("upper", np.float64), ("lower", np.float64), ("bou", np.float64),
+             ("int", np.float64), ("perm", np.int32), ("inv", np.float64), ("invDims", np.int32)]
+
+    def debug_get(self, lev, name):
+        """HOST copy of one array of coarse level lev (b200ldu_gamg_debug_get)"""
+        what = [k for k, _ in self.DEBUG].index(name)
+        n = lib().b200ldu_gamg_debug_get(self.h, lev, what, None, 0)
+        if n < 0:
+            check(int(n))
+        out = np.zeros(max(n, 1), dtype=self.DEBUG[what][1])
+        check(int(min(0, lib().b200ldu_gamg_debug_get(self.h, lev, what, _hp(out), n))))
+        return out[:n]
+
+    def level_addressing(self, lev):
+        """dict(owner, neighbour, faceRestrict, faceFlip) of coarse level lev; also on a host-only hierarchy"""
+        return {k: self.debug_get(lev, k) for k in ("owner", "neighbour", "faceRestrict", "faceFlip")}
+
+    def level_state(self, lev):
+        """the addressing, the last solve's coarse coefficients (lower None when that matrix was symmetric), the
+        interface coefficients and the banded permutation of coarse level lev"""
+        out = self.level_addressing(lev)
+        for k in ("diag", "upper", "lower", "bou", "int", "perm"):
+            out[k] = self.debug_get(lev, k)
+        if out["lower"].size == 0 and out["upper"].size:
+            out["lower"] = None
+        return out
+
+    def coarsest_inverse(self):
+        """(rows, N, offset): this rank's rows of the inverse of the coarsest matrix as the last solve uploaded
+        them -- banded rows x global banded columns -- the global size and this rank's first row"""
+        lev = self.nLevels - 1
+        N, off, n = (int(v) for v in self.debug_get(lev, "invDims"))
+        return self.debug_get(lev, "inv").reshape(n, N), N, off
 
     def close(self):
         if self.h:

@@ -25,6 +25,7 @@
 // master; here every rank holds its own rows of the inverse and the right-hand sides are
 // all-gathered through peer memory inside the solve kernel).
 #include <algorithm>
+#include <climits>
 #include <cmath>
 
 #include "comm.h"
@@ -47,8 +48,12 @@ struct GamgHostLevel {
 };
 
 struct GamgLevel {
-    int nCoarse = 0, nCoarseFaces = 0;
+    int nCoarse = 0, nCoarseFaces = 0, nFineFaces = 0;
     std::vector<int> restrictAddr;      // fine cell -> coarse cell (caller orders)
+    // a host-only hierarchy keeps the coarse addressing and face maps here (b200ldu_gamg_debug_get); a device level
+    // has them in addr and in the face maps below
+    std::vector<int> hOwner, hNeigh, hFaceRestrict;
+    std::vector<unsigned char> hFaceFlip;
     b200ldu_addr *addr = nullptr;       // coarse level addressing (banded layout built)
     b200ldu_matrix *mat = nullptr;      // coarse level matrix (values refreshed every solve)
     // device maps, banded vector space
@@ -80,6 +85,9 @@ struct b200ldu_gamg {
     std::vector<GamgLevel> lev;
     double *d_inv = nullptr; // this rank's rows of the inverse of the (global) coarsest matrix
     int invN = 0;            // global size of the coarsest system
+    int invOff = 0;          // this rank's first row of it
+    bool built = false;      // the coarse matrices of a solve are in the levels' d_diag / d_upper / d_lower / d_bou / d_int
+    bool builtAsym = false;  // ... with d_lower filled
     // multi-rank coarsest solve
     std::vector<int> coarsestCounts, coarsestOffs, coarsestNbrCell;
     int nMaxCoarsest = 0;
@@ -379,10 +387,17 @@ static int level_upload(b200ldu_gamg *g, const b200ldu_addr *fineAddr, GamgHostL
     L.nCoarse = H.nCoarse;
     L.nCoarseFaces = H.nCoarseFaces;
     L.nCoarsePF = H.nCoarsePF;
+    L.nFineFaces = H.nFineFaces;
     L.restrictAddr = std::move(H.map);
     L.cPatchStart = std::move(H.cPatchStart);
     L.cFaceCells = std::move(H.cFaceCells);
-    if (a->hostOnly) return B200LDU_OK;
+    if (a->hostOnly) {
+        L.hOwner = std::move(H.cOwner);
+        L.hNeigh = std::move(H.cNeigh);
+        L.hFaceRestrict = std::move(H.faceRestrict);
+        L.hFaceFlip = std::move(H.faceFlip);
+        return B200LDU_OK;
+    }
     const int nPatches = a->nPatches, nCoarse = H.nCoarse;
     TRY(b200ldu_addr_create(a->ctx, nCoarse, H.nCoarseFaces, H.cOwner.data(), H.cNeigh.data(), nPatches,
                             nPatches ? L.cPatchStart.data() : nullptr, nPatches ? L.cFaceCells.data() : nullptr,
@@ -512,6 +527,85 @@ extern "C" int b200ldu_gamg_restrict_addr(const b200ldu_gamg *g, int lev, int *o
     if (!g || lev < 0 || lev >= g->nLevels || !out_h) return B200LDU_EINVAL;
     memcpy(out_h, g->lev[lev].restrictAddr.data(), sizeof(int) * g->lev[lev].restrictAddr.size());
     return B200LDU_OK;
+}
+
+// Read-back for parity tests: HOST copies of what a level holds.  Addressing and face maps come from the arrays the
+// kernels read (the coarse addressing, the coarse face -> fine faces and coarse cell -> collapsed faces maps inverted
+// back to caller order), coefficients from the last solve's coarse matrices.  Read-only: it waits for the context
+// stream and changes nothing a later solve sees.
+extern "C" long long b200ldu_gamg_debug_get(const b200ldu_gamg *g, int lev, int what, void *out_h, long long cap)
+{
+    if (!g || lev < 0 || lev >= g->nLevels || what < 0 || what > B200LDU_GAMG_INV_DIMS) return B200LDU_EINVAL;
+    const GamgLevel &L = g->lev[lev];
+    const bool host = g->finest->hostOnly;
+    const bool coarsest = lev == g->nLevels - 1;
+    auto give = [&](const void *src, size_t elem, long long n) -> long long {
+        if (out_h && n > 0) memcpy(out_h, src, elem * (size_t)std::min(n, std::max(cap, 0LL)));
+        return n;
+    };
+    const bool coeffs = what >= B200LDU_GAMG_DIAG && what <= B200LDU_GAMG_INT;
+    const bool inv = what == B200LDU_GAMG_INV || what == B200LDU_GAMG_INV_DIMS;
+    if (host && (coeffs || inv || what == B200LDU_GAMG_PERM)) return B200LDU_EINVAL;
+    if (coeffs && !g->built) return B200LDU_EINVAL;
+    if (inv && (!coarsest || !g->invN)) return B200LDU_EINVAL;
+    if (!host) {
+        if (cudaSetDevice(g->finest->ctx->device) != cudaSuccess) return B200LDU_ECUDA;
+        if (cudaStreamSynchronize(g->finest->ctx->stream) != cudaSuccess) return B200LDU_ECUDA;
+    }
+    auto fetch = [&](const void *d, size_t bytes, void *h) {
+        return bytes == 0 || cudaMemcpy(h, d, bytes, cudaMemcpyDeviceToHost) == cudaSuccess;
+    };
+    switch (what) {
+    case B200LDU_GAMG_OWNER: return host ? give(L.hOwner.data(), 4, L.nCoarseFaces) : give(L.addr->l.data(), 4, L.nCoarseFaces);
+    case B200LDU_GAMG_NEIGHBOUR: return host ? give(L.hNeigh.data(), 4, L.nCoarseFaces) : give(L.addr->u.data(), 4, L.nCoarseFaces);
+    case B200LDU_GAMG_FACE_RESTRICT:
+    case B200LDU_GAMG_FACE_FLIP: {
+        const bool flip = what == B200LDU_GAMG_FACE_FLIP;
+        std::vector<int> v(std::max(L.nFineFaces, 1), 0);
+        if (host) {
+            for (int f = 0; f < L.nFineFaces; f++) v[f] = flip ? L.hFaceFlip[f] : L.hFaceRestrict[f];
+            return give(v.data(), 4, L.nFineFaces);
+        }
+        // every fine face appears once in the two maps; a face in neither stays at the marker INT_MIN
+        std::vector<int> fs(L.nCoarseFaces + 1), ds(L.nCoarse + 1);
+        if (!fetch(L.d_faceChildStart, 4 * fs.size(), fs.data()) || !fetch(L.d_diagFaceStart, 4 * ds.size(), ds.data()))
+            return B200LDU_ECUDA;
+        std::vector<int> fi(std::max(fs.back(), 1)), di(std::max(ds.back(), 1));
+        if (!fetch(L.d_faceChild, 4 * (size_t)fs.back(), fi.data()) || !fetch(L.d_diagFace, 4 * (size_t)ds.back(), di.data()))
+            return B200LDU_ECUDA;
+        std::fill(v.begin(), v.end(), INT_MIN);
+        for (int F = 0; F < L.nCoarseFaces; F++)
+            for (int k = fs[F]; k < fs[F + 1]; k++) v[fi[k] >> 1] = flip ? (fi[k] & 1) : F;
+        for (int C = 0; C < L.nCoarse; C++)
+            for (int k = ds[C]; k < ds[C + 1]; k++) v[di[k]] = flip ? 0 : -(C + 1);
+        return give(v.data(), 4, L.nFineFaces);
+    }
+    case B200LDU_GAMG_DIAG:
+    case B200LDU_GAMG_UPPER:
+    case B200LDU_GAMG_LOWER:
+    case B200LDU_GAMG_BOU:
+    case B200LDU_GAMG_INT: {
+        if (what == B200LDU_GAMG_LOWER && !g->builtAsym) return 0; // a symmetric matrix has no lower of its own
+        const double *src = what == B200LDU_GAMG_DIAG ? L.d_diag : what == B200LDU_GAMG_UPPER ? L.d_upper
+                          : what == B200LDU_GAMG_LOWER ? L.d_lower : what == B200LDU_GAMG_BOU ? L.d_bou : L.d_int;
+        const long long n = what == B200LDU_GAMG_DIAG ? L.nCoarse : what <= B200LDU_GAMG_LOWER ? L.nCoarseFaces : L.nCoarsePF;
+        std::vector<double> v(std::max(n, 1LL));
+        if (!fetch(src, 8 * (size_t)n, v.data())) return B200LDU_ECUDA;
+        return give(v.data(), 8, n);
+    }
+    case B200LDU_GAMG_PERM: return give(L.addr->perm_h.data(), 4, L.nCoarse);
+    case B200LDU_GAMG_INV: {
+        const long long n = (long long)L.nCoarse * g->invN;
+        std::vector<double> v(std::max(n, 1LL));
+        if (!fetch(g->d_inv, 8 * (size_t)n, v.data())) return B200LDU_ECUDA;
+        return give(v.data(), 8, n);
+    }
+    case B200LDU_GAMG_INV_DIMS: {
+        int dims[3] = {g->invN, g->invOff, L.nCoarse};
+        return give(dims, 4, 3);
+    }
+    }
+    return B200LDU_EINVAL;
 }
 
 // ---------------------------------------------------------------------------
@@ -722,6 +816,8 @@ static int gamg_build_matrices(Solve &S, b200ldu_gamg *g)
         b200_set_error("GAMG: matrix coefficients not set");
         return B200LDU_EINVAL;
     }
+    g->built = false;
+    g->builtAsym = fl != nullptr;
     for (int k = 0; k < g->nLevels; k++) {
         GamgLevel &L = g->lev[k];
         TRY(launch(S.ctx, agg_diag_kernel, L.nCoarse, 256, L.nCoarse, L.d_cellChildStart, L.d_cellChild,
@@ -740,7 +836,60 @@ static int gamg_build_matrices(Solve &S, b200ldu_gamg *g)
         fu = L.d_upper;
         fl = fl ? L.d_lower : nullptr;
     }
+    g->built = true;
     return B200LDU_OK;
+}
+
+// Partial-pivot Gauss-Jordan inverse of the row-major N x N matrix A (destroyed) into I: the first row of the largest
+// magnitude in column k is the pivot row.  Returns the number of row swaps, or -1 when a column has no nonzero pivot.
+static int gauss_jordan_inverse(std::vector<double> &A, int N, std::vector<double> &I)
+{
+    I.assign((size_t)N * N, 0.0);
+    int swaps = 0;
+    for (int c = 0; c < N; c++) I[(size_t)c * N + c] = 1.0;
+    for (int k = 0; k < N; k++) {
+        int p = k;
+        double mx = fabs(A[(size_t)k * N + k]);
+        for (int i = k + 1; i < N; i++)
+            if (fabs(A[(size_t)i * N + k]) > mx) {
+                mx = fabs(A[(size_t)i * N + k]);
+                p = i;
+            }
+        if (mx == 0.0) return -1;
+        if (p != k) {
+            swaps++;
+            for (int j = 0; j < N; j++) {
+                std::swap(A[(size_t)k * N + j], A[(size_t)p * N + j]);
+                std::swap(I[(size_t)k * N + j], I[(size_t)p * N + j]);
+            }
+        }
+        double piv = 1.0 / A[(size_t)k * N + k];
+        for (int j = 0; j < N; j++) {
+            A[(size_t)k * N + j] *= piv;
+            I[(size_t)k * N + j] *= piv;
+        }
+        for (int i = 0; i < N; i++) {
+            if (i == k) continue;
+            double fct = A[(size_t)i * N + k];
+            if (fct == 0.0) continue;
+            for (int j = 0; j < N; j++) {
+                A[(size_t)i * N + j] -= fct * A[(size_t)k * N + j];
+                I[(size_t)i * N + j] -= fct * I[(size_t)k * N + j];
+            }
+        }
+    }
+    return swaps;
+}
+
+// the host inverse on its own, for the CPU test-suite
+extern "C" int b200ldu_gamg_debug_invert(int N, const double *A_h, double *inv_h)
+{
+    if (N < 1 || !A_h || !inv_h) return B200LDU_EINVAL;
+    std::vector<double> A(A_h, A_h + (size_t)N * N), I;
+    int swaps = gauss_jordan_inverse(A, N, I);
+    if (swaps < 0) return B200LDU_EINVAL;
+    memcpy(inv_h, I.data(), sizeof(double) * (size_t)N * N);
+    return swaps;
 }
 
 // Inverse of the coarsest matrix on the host (partial-pivot Gauss-Jordan), standing in for
@@ -804,42 +953,14 @@ static int gamg_coarsest_inverse(Solve &S, b200ldu_gamg *g)
                 memcpy(&A[(size_t)(g->coarsestOffs[r] + i) * N], &all[((size_t)r * nMax + i) * N], sizeof(double) * N);
     } else
         A = rows;
-    std::vector<double> I((size_t)N * N, 0.0);
-    for (int c = 0; c < N; c++) I[(size_t)c * N + c] = 1.0;
-    for (int k = 0; k < N; k++) {
-        int p = k;
-        double mx = fabs(A[(size_t)k * N + k]);
-        for (int i = k + 1; i < N; i++)
-            if (fabs(A[(size_t)i * N + k]) > mx) {
-                mx = fabs(A[(size_t)i * N + k]);
-                p = i;
-            }
-        if (mx == 0.0) {
-            b200_set_error("GAMG: coarsest-level matrix is singular");
-            return B200LDU_EINVAL;
-        }
-        if (p != k)
-            for (int j = 0; j < N; j++) {
-                std::swap(A[(size_t)k * N + j], A[(size_t)p * N + j]);
-                std::swap(I[(size_t)k * N + j], I[(size_t)p * N + j]);
-            }
-        double piv = 1.0 / A[(size_t)k * N + k];
-        for (int j = 0; j < N; j++) {
-            A[(size_t)k * N + j] *= piv;
-            I[(size_t)k * N + j] *= piv;
-        }
-        for (int i = 0; i < N; i++) {
-            if (i == k) continue;
-            double fct = A[(size_t)i * N + k];
-            if (fct == 0.0) continue;
-            for (int j = 0; j < N; j++) {
-                A[(size_t)i * N + j] -= fct * A[(size_t)k * N + j];
-                I[(size_t)i * N + j] -= fct * I[(size_t)k * N + j];
-            }
-        }
+    std::vector<double> I;
+    if (gauss_jordan_inverse(A, N, I) < 0) {
+        b200_set_error("GAMG: coarsest-level matrix is singular");
+        return B200LDU_EINVAL;
     }
     TRY(g->mem.slot(GAMG_INV, g->d_inv, (size_t)std::max(n, 1) * N));
     g->invN = N;
+    g->invOff = off;
     CUDA_TRY(cudaMemcpyAsync(g->d_inv, &I[(size_t)off * N], sizeof(double) * (size_t)n * N, cudaMemcpyHostToDevice, st));
     std::vector<int> meta(64, 0);
     if (R > 1 && !ctx->p2p) {
