@@ -225,6 +225,36 @@ enum {
     B200LDU_GAMG_PERM, B200LDU_GAMG_INV, B200LDU_GAMG_INV_DIMS
 };
 long long b200ldu_gamg_debug_get(const b200ldu_gamg *g, int lev, int what, void *out_h, long long cap);
+/* Trace of a matrix handle's global sums, for tests that run a solve in lockstep with a CPU restatement.
+ * b200ldu_matrix_debug_trace(m, cap) arms it for the handle's later solves (cap records; 0 disarms it).  Every scalar
+ * step of a solve then stores one record, in step order: what it summed and the per-CTA partials it summed them from.
+ * Unarmed, a solve does exactly what it does without this entry point.  b200ldu_matrix_debug_get(m, what, out_h, cap)
+ * copies up to cap doubles of the last solve's trace to out_h and returns how many there are; it waits for the
+ * context's stream and changes nothing:
+ *   TRACE_RECORDS   double[nRec * 16]  per record: kind (B200LDU_STEP_*), NRED, nPartials, nIterations before the
+ *                                      step, sum[0..7] (sum[k], k < NRED, as the step's logic saw it), 4 unused
+ *   TRACE_PARTIALS  double[nRec * P]   per record: partials[p * NRED + k], p < nPartials (P: the return value / nRec)
+ *   TRACE_SCALARS   double[12]         wArA, wApA, alpha, beta, omega, rA0rA, tAtA, tAsA, normFactor, bodies,
+ *                                      psiBodies, and the number of steps the solve ran (more than cap: records lost)
+ * nRec = min(steps, cap). */
+enum { B200LDU_TRACE_RECORDS, B200LDU_TRACE_PARTIALS, B200LDU_TRACE_SCALARS };
+enum {
+    B200LDU_STEP_OTHER,     /* a step without a name (GAMG) */
+    B200LDU_STEP_INIT,      /* sum|b - A psi|, sum psi */
+    B200LDU_STEP_NORM,      /* normFactor */
+    B200LDU_STEP_BETA,      /* PCG <w,r> / PBiCG <wA,rT> (operation list) */
+    B200LDU_STEP_ALPHA,     /* PCG <Ap,p> / PBiCG <A pA,pT> (operation list) */
+    B200LDU_STEP_END,       /* sum|r| closing an iteration (operation list, PBiCGStab, smoothSolver) */
+    B200LDU_STEP_PCG_A,     /* fused PCG sweep A: <z,r>, sum|r| of the previous body */
+    B200LDU_STEP_PCG_B,     /* fused PCG sweep B: <Ap,p> */
+    B200LDU_STEP_PCG_CLOSE, /* fused PCG close: sum|r| of the last body */
+    B200LDU_STEP_RHO,       /* PBiCGStab <rA0,rA> */
+    B200LDU_STEP_RA0AYA,    /* PBiCGStab <rA0,AyA> */
+    B200LDU_STEP_SMAG,      /* PBiCGStab sum|sA| */
+    B200LDU_STEP_OMEGA      /* PBiCGStab <tA,tA>, <tA,sA> */
+};
+int b200ldu_matrix_debug_trace(b200ldu_matrix *m, int cap);
+long long b200ldu_matrix_debug_get(const b200ldu_matrix *m, int what, double *out_h, long long cap);
 /* The host inverse a GAMG solve uploads for its coarsest level (partial-pivot Gauss-Jordan), on its own: inv_h = A_h^-1,
  * both HOST row-major N x N.  Returns the number of row swaps, or B200LDU_EINVAL for a singular A_h.  No GPU. */
 int b200ldu_gamg_debug_invert(int N, const double *A_h, double *inv_h);

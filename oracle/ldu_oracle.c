@@ -394,6 +394,27 @@ double orc_gsummag(const double *x, int n, const orc_comm *comm)
     return s;
 }
 
+/* the lockstep hook (ldu_oracle.h): per thread, so concurrent tests do not see each other's */
+static _Thread_local orc_reduce_fn hookFn;
+static _Thread_local void *hookCtx;
+static _Thread_local int stagedAinv;
+
+void orc_set_reduce_hook(orc_reduce_fn fn, void *ctx)
+{
+    hookFn = fn;
+    hookCtx = ctx;
+}
+
+void orc_set_staged_ainv(int on) { stagedAinv = on; }
+
+/* a global sum at a named call site: the oracle's own value, or the hook's when it is armed */
+static double site_sum(int site, int iter, int op, const double *x, const double *y, int n, const orc_comm *comm)
+{
+    double s = op == ORC_RED_PROD ? orc_gsumprod(x, y, n, comm) : op == ORC_RED_MAG ? orc_gsummag(x, n, comm)
+                                                                                 : orc_gsum(x, n, comm);
+    return hookFn ? hookFn(hookCtx, site, iter, op, x, y, n, s) : s;
+}
+
 /* normFactor: LDU/lduMatrix/lduMatrixSolver.C:183-236 */
 double orc_normFactor(const orc_matrix *m, const double *psi, const double *source,
                       const double *Apsi, double *tmp, const orc_comm *comm)
@@ -401,7 +422,7 @@ double orc_normFactor(const orc_matrix *m, const double *psi, const double *sour
     int n = m->a->nCells;
     orc_sumA(m, tmp);
     /* gAverage: gpuFieldCommonFunctions.C:611-635 -- global sum / global size */
-    double s = orc_gsum(psi, n, comm);
+    double s = site_sum(ORC_SITE_SUMPSI, 0, ORC_RED_SUM, psi, NULL, n, comm);
     double cnt = (comm && comm->nCellsGlobal) ? (double)comm->nCellsGlobal : (double)n;
     double avg = s / cnt;
     double factor = 0;
@@ -410,6 +431,16 @@ double orc_normFactor(const orc_matrix *m, const double *psi, const double *sour
         factor += fabs(Apsi[c] - t) + fabs(source[c] - t);
     }
     if (comm && comm->sum) comm->sum(comm->ctx, &factor, 1);
+    if (hookFn) {
+        double *terms = (double *)malloc(sizeof(double) * (size_t)(n > 0 ? 2 * n : 1));
+        for (int c = 0; c < n; c++) {
+            double t = avg * tmp[c];
+            terms[2 * c] = Apsi[c] - t;
+            terms[2 * c + 1] = source[c] - t;
+        }
+        factor = hookFn(hookCtx, ORC_SITE_NORMFACTOR, 0, ORC_RED_MAG, terms, NULL, 2 * n, factor);
+        free(terms);
+    }
     return factor + ORC_SMALL;
 }
 
@@ -435,13 +466,13 @@ void orc_precondition(const orc_matrix *m, int kind, int transpose, const double
             double out = 0.0;
             for (int f = a->ownerStart[c]; f < a->ownerStart[c + 1]; f++) {
                 int nb = a->u[f];
-                double p = (U[f] * rD[nb]) * r[nb];
+                double p = stagedAinv ? U[f] * (rD[nb] * r[nb]) : (U[f] * rD[nb]) * r[nb];
                 out = out + p;
             }
             for (int k = a->losortStart[c]; k < a->losortStart[c + 1]; k++) {
                 int f = a->losort[k];
                 int nb = a->l[f];
-                double p = (L[f] * rD[nb]) * r[nb];
+                double p = stagedAinv ? L[f] * (rD[nb] * r[nb]) : (L[f] * rD[nb]) * r[nb];
                 out = out + p;
             }
             w[c] = rD[c] * (r[c] - out);
@@ -547,16 +578,17 @@ static int orc_pcg(const orc_matrix *m, int pk, const orc_controls *c, double *p
     for (int i = 0; i < n; i++) rA[i] = source[i] - wA[i];
     double normFactor = orc_normFactor(m, psi, source, wA, pA, comm);
     perf->normFactor = normFactor;
-    perf->initialResidual = orc_gsummag(rA, n, comm) / normFactor;
+    perf->initialResidual = site_sum(ORC_SITE_SUMMAG0, 0, ORC_RED_MAG, rA, NULL, n, comm) / normFactor;
     perf->finalResidual = perf->initialResidual;
     hist_put(hist, cap, 0, perf->finalResidual);
 
     if (c->minIter > 0 || !orc_converged(perf, c->tolerance, c->relTol)) {
         double *rD = make_rD(m);
         do {
+            const int it = perf->nIterations;
             wArAold = wArA;
             orc_precondition(m, pk, 0, rD, rA, wA);
-            wArA = orc_gsumprod(wA, rA, n, comm);
+            wArA = site_sum(ORC_SITE_WARA, it, ORC_RED_PROD, wA, rA, n, comm);
             if (perf->nIterations == 0) {
                 memcpy(pA, wA, sizeof(double) * (size_t)n);
             } else {
@@ -564,12 +596,12 @@ static int orc_pcg(const orc_matrix *m, int pk, const orc_controls *c, double *p
                 for (int i = 0; i < n; i++) pA[i] = fma(beta, pA[i], wA[i]);
             }
             orc_amul(m, pA, wA, comm);
-            double wApA = orc_gsumprod(wA, pA, n, comm);
+            double wApA = site_sum(ORC_SITE_WAPA, it, ORC_RED_PROD, wA, pA, n, comm);
             if (orc_singular(perf, fabs(wApA) / normFactor)) break;
             double alpha = wArA / wApA;
             for (int i = 0; i < n; i++) psi[i] = fma(alpha, pA[i], psi[i]);
             for (int i = 0; i < n; i++) rA[i] = fma(-alpha, wA[i], rA[i]);
-            perf->finalResidual = orc_gsummag(rA, n, comm) / normFactor;
+            perf->finalResidual = site_sum(ORC_SITE_SUMMAG, it, ORC_RED_MAG, rA, NULL, n, comm) / normFactor;
             hist_put(hist, cap, perf->nIterations + 1, perf->finalResidual);
         } while ((perf->nIterations++ < c->maxIter &&
                   !orc_converged(perf, c->tolerance, c->relTol)) ||
@@ -598,17 +630,18 @@ static int orc_pbicg(const orc_matrix *m, int pk, const orc_controls *c, double 
     for (int i = 0; i < n; i++) rT[i] = source[i] - wT[i];
     double normFactor = orc_normFactor(m, psi, source, wA, pA, comm);
     perf->normFactor = normFactor;
-    perf->initialResidual = orc_gsummag(rA, n, comm) / normFactor;
+    perf->initialResidual = site_sum(ORC_SITE_SUMMAG0, 0, ORC_RED_MAG, rA, NULL, n, comm) / normFactor;
     perf->finalResidual = perf->initialResidual;
     hist_put(hist, cap, 0, perf->finalResidual);
 
     if (c->minIter > 0 || !orc_converged(perf, c->tolerance, c->relTol)) {
         double *rD = make_rD(m);
         do {
+            const int it = perf->nIterations;
             wArTold = wArT;
             orc_precondition(m, pk, 0, rD, rA, wA);
             orc_precondition(m, pk, 1, rD, rT, wT);
-            wArT = orc_gsumprod(wA, rT, n, comm);
+            wArT = site_sum(ORC_SITE_WART, it, ORC_RED_PROD, wA, rT, n, comm);
             if (perf->nIterations == 0) {
                 memcpy(pA, wA, sizeof(double) * (size_t)n);
                 memcpy(pT, wT, sizeof(double) * (size_t)n);
@@ -619,13 +652,13 @@ static int orc_pbicg(const orc_matrix *m, int pk, const orc_controls *c, double 
             }
             orc_amul(m, pA, wA, comm);
             orc_tmul(m, pT, wT, comm);
-            double wApT = orc_gsumprod(wA, pT, n, comm);
+            double wApT = site_sum(ORC_SITE_WAPT, it, ORC_RED_PROD, wA, pT, n, comm);
             if (orc_singular(perf, fabs(wApT) / normFactor)) break;
             double alpha = wArT / wApT;
             for (int i = 0; i < n; i++) psi[i] = fma(alpha, pA[i], psi[i]);
             for (int i = 0; i < n; i++) rA[i] = fma(-alpha, wA[i], rA[i]);
             for (int i = 0; i < n; i++) rT[i] = fma(-alpha, wT[i], rT[i]);
-            perf->finalResidual = orc_gsummag(rA, n, comm) / normFactor;
+            perf->finalResidual = site_sum(ORC_SITE_SUMMAG, it, ORC_RED_MAG, rA, NULL, n, comm) / normFactor;
             hist_put(hist, cap, perf->nIterations + 1, perf->finalResidual);
         } while ((perf->nIterations++ < c->maxIter &&
                   !orc_converged(perf, c->tolerance, c->relTol)) ||
@@ -654,7 +687,7 @@ static int orc_pbicgstab(const orc_matrix *m, int pk, const orc_controls *c, dou
     for (int i = 0; i < n; i++) rA[i] = source[i] - yA[i];
     double normFactor = orc_normFactor(m, psi, source, yA, pA, comm);
     perf->normFactor = normFactor;
-    perf->initialResidual = orc_gsummag(rA, n, comm) / normFactor;
+    perf->initialResidual = site_sum(ORC_SITE_SUMMAG0, 0, ORC_RED_MAG, rA, NULL, n, comm) / normFactor;
     perf->finalResidual = perf->initialResidual;
     hist_put(hist, cap, 0, perf->finalResidual);
 
@@ -665,8 +698,9 @@ static int orc_pbicgstab(const orc_matrix *m, int pk, const orc_controls *c, dou
         double rA0rA = 0, alpha = 0, omega = 0;
         int early = 0;
         do {
+            const int it = perf->nIterations;
             double rA0rAold = rA0rA;
-            rA0rA = orc_gsumprod(rA0, rA, n, comm);
+            rA0rA = site_sum(ORC_SITE_RA0RA, it, ORC_RED_PROD, rA0, rA, n, comm);
             if (orc_singular(perf, fabs(rA0rA))) break;
             if (perf->nIterations == 0) {
                 memcpy(pA, rA, sizeof(double) * (size_t)n);
@@ -680,10 +714,10 @@ static int orc_pbicgstab(const orc_matrix *m, int pk, const orc_controls *c, dou
             }
             orc_precondition(m, pk, 0, rD, pA, yA);
             orc_amul(m, yA, AyA, comm);
-            double rA0AyA = orc_gsumprod(rA0, AyA, n, comm);
+            double rA0AyA = site_sum(ORC_SITE_RA0AYA, it, ORC_RED_PROD, rA0, AyA, n, comm);
             alpha = rA0rA / rA0AyA;
             for (int i = 0; i < n; i++) sA[i] = fma(-alpha, AyA[i], rA[i]);
-            perf->finalResidual = orc_gsummag(sA, n, comm) / normFactor;
+            perf->finalResidual = site_sum(ORC_SITE_SUMMAGS, it, ORC_RED_MAG, sA, NULL, n, comm) / normFactor;
             if (orc_converged(perf, c->tolerance, c->relTol)) {
                 for (int i = 0; i < n; i++) psi[i] = fma(alpha, yA[i], psi[i]);
                 perf->nIterations++;
@@ -693,15 +727,15 @@ static int orc_pbicgstab(const orc_matrix *m, int pk, const orc_controls *c, dou
             }
             orc_precondition(m, pk, 0, rD, sA, zA);
             orc_amul(m, zA, tA, comm);
-            double tAtA = orc_gsumprod(tA, tA, n, comm);
-            omega = orc_gsumprod(tA, sA, n, comm) / tAtA;
+            double tAtA = site_sum(ORC_SITE_TATA, it, ORC_RED_PROD, tA, tA, n, comm);
+            omega = site_sum(ORC_SITE_TASA, it, ORC_RED_PROD, tA, sA, n, comm) / tAtA;
             for (int i = 0; i < n; i++) psi[i] = fma(alpha, yA[i], psi[i]);
             {
                 const double *second = c->bicgstabRefQuirk ? yA : zA;
                 for (int i = 0; i < n; i++) psi[i] = fma(omega, second[i], psi[i]);
             }
             for (int i = 0; i < n; i++) rA[i] = fma(-omega, tA[i], sA[i]);
-            perf->finalResidual = orc_gsummag(rA, n, comm) / normFactor;
+            perf->finalResidual = site_sum(ORC_SITE_SUMMAG, it, ORC_RED_MAG, rA, NULL, n, comm) / normFactor;
             hist_put(hist, cap, perf->nIterations + 1, perf->finalResidual);
         } while ((perf->nIterations++ < c->maxIter &&
                   !orc_converged(perf, c->tolerance, c->relTol)) ||
@@ -737,7 +771,7 @@ static int orc_smooth_solver(const orc_matrix *m, const orc_controls *c, double 
     double normFactor = orc_normFactor(m, psi, source, Apsi, tmp, comm);
     perf->normFactor = normFactor;
     for (int i = 0; i < n; i++) tmp[i] = source[i] - Apsi[i];
-    perf->initialResidual = orc_gsummag(tmp, n, comm) / normFactor;
+    perf->initialResidual = site_sum(ORC_SITE_SUMMAG0, 0, ORC_RED_MAG, tmp, NULL, n, comm) / normFactor;
     perf->finalResidual = perf->initialResidual;
     hist_put(hist, cap, 0, perf->finalResidual);
     if (c->minIter > 0 || !orc_converged(perf, c->tolerance, c->relTol)) {
@@ -745,7 +779,7 @@ static int orc_smooth_solver(const orc_matrix *m, const orc_controls *c, double 
         do {
             orc_jacobi_smooth(m, c->omega, psi, source, c->nSweeps, comm);
             orc_residual(m, psi, source, tmp, comm);
-            perf->finalResidual = orc_gsummag(tmp, n, comm) / normFactor;
+            perf->finalResidual = site_sum(ORC_SITE_SUMMAG, k, ORC_RED_MAG, tmp, NULL, n, comm) / normFactor;
             hist_put(hist, cap, ++k, perf->finalResidual);
         } while (((perf->nIterations += c->nSweeps) < c->maxIter &&
                   !orc_converged(perf, c->tolerance, c->relTol)) ||

@@ -149,6 +149,24 @@ void orc_precondition(const orc_matrix *m, int kind, int transpose, const double
 void orc_jacobi_smooth(const orc_matrix *m, double omega, double *psi, const double *source,
                        int nSweeps, const orc_comm *comm);
 
+/* ---- lockstep with a device solve (tests only; off by default, per thread, single rank) ----
+ * An armed reduction hook is called at every global sum of the Krylov solvers, of smoothSolver and of normFactor,
+ * after the oracle has formed its own value, and the solve goes on with the value it returns.  site names the
+ * call (ORC_SITE_*), iter the iteration body it belongs to (0-based; 0 for the sums before the first body), op the
+ * terms: ORC_RED_SUM x[i], ORC_RED_PROD x[i]*y[i] (each product rounded), ORC_RED_MAG |x[i]|.  normFactor hands its
+ * 2n terms |Apsi - avg*sumA|, |source - avg*sumA| as x with ORC_RED_MAG.  fn = NULL disarms it. */
+enum {
+    ORC_SITE_SUMPSI, ORC_SITE_NORMFACTOR, ORC_SITE_SUMMAG0, ORC_SITE_WARA, ORC_SITE_WAPA, ORC_SITE_SUMMAG,
+    ORC_SITE_WART, ORC_SITE_WAPT, ORC_SITE_RA0RA, ORC_SITE_RA0AYA, ORC_SITE_SUMMAGS, ORC_SITE_TATA, ORC_SITE_TASA
+};
+enum { ORC_RED_SUM, ORC_RED_PROD, ORC_RED_MAG };
+typedef double (*orc_reduce_fn)(void *ctx, int site, int iter, int op, const double *x, const double *y, int n,
+                                double own);
+void orc_set_reduce_hook(orc_reduce_fn fn, void *ctx);
+/* AINV with the device's association, rD[c]*r[c] formed first and then multiplied by the coefficient (DESIGN.md
+ * section 2, exception (i)); 0 (default): the reference's (coeff*rD[c])*r[c].  Per thread. */
+void orc_set_staged_ainv(int on);
+
 /* ---- solvers; hist (may be NULL) receives the normalised residual after every
  * iteration body: hist[0] = initial, hist[k] = after k-th body ---- */
 int orc_solve(const orc_matrix *m, const char *solver, const char *precondOrSmoother,

@@ -52,6 +52,12 @@ class Perf(C.Structure):
 HALO_CB = C.CFUNCTYPE(None, C.c_void_p, c_dp, c_dp, C.c_int, C.c_int, c_ip)
 SUM_CB = C.CFUNCTYPE(None, C.c_void_p, c_dp, C.c_int)
 GATHER_CB = C.CFUNCTYPE(None, C.c_void_p, c_dp, C.c_int, c_dp)
+REDUCE_CB = C.CFUNCTYPE(C.c_double, C.c_void_p, C.c_int, C.c_int, C.c_int, c_dp, c_dp, C.c_int, C.c_double)
+
+# call sites of the reduction hook, in the order of ORC_SITE_* (ldu_oracle.h), and its term kinds (ORC_RED_*)
+SITES = ("sumPsi", "normFactor", "sumMag0", "wArA", "wApA", "sumMag", "wArT", "wApT", "rA0rA", "rA0AyA", "sumMagS",
+         "tAtA", "tAsA")
+RED_OPS = ("sum", "prod", "mag")
 
 
 class Comm(C.Structure):
@@ -115,6 +121,8 @@ def lib():
         L.orc_gamg_set_coarsest_inverse.argtypes = [C.c_void_p, c_dp, c_ip, C.c_int]
         L.orc_gamg_set_scale_order.argtypes = [C.c_void_p, C.c_int]
         L.orc_addr_npatches.argtypes = [C.c_void_p]
+        L.orc_set_reduce_hook.argtypes = [REDUCE_CB, C.c_void_p]
+        L.orc_set_staged_ainv.argtypes = [C.c_int]
         for nm in ("orc_addr_patch_start", "orc_addr_face_cells"):
             getattr(L, nm).restype = c_ip
             getattr(L, nm).argtypes = [C.c_void_p]
@@ -267,6 +275,33 @@ class PyComm:
 
 def _commp(comm):
     return None if comm is None else comm.ptr()
+
+
+class ReduceHook:
+    """Lockstep with a device solve, for the calling thread while the block runs (single rank):
+    fn(site, it, op, x, y, own) -> the value the oracle goes on with, at every global sum of the Krylov solvers,
+    smoothSolver and normFactor.  site is a name of SITES, it the iteration body (0 for the sums before the first),
+    op "sum" / "prod" / "mag" with the terms x[i], x[i]*y[i] or |x[i]|; x and y are views of the oracle's own
+    vectors (y None unless op is "prod"), own is the oracle's sum.  staged_ainv: AINV with the device's association
+    (orc_set_staged_ainv) for as long as the hook is armed."""
+
+    def __init__(self, fn, staged_ainv=False):
+        def _cb(ctx, site, it, op, x, y, n, own):
+            xv = np.ctypeslib.as_array(x, (n,)) if n > 0 else np.zeros(0)
+            yv = np.ctypeslib.as_array(y, (n,)) if (y and n > 0) else None
+            return float(fn(SITES[site], it, RED_OPS[op], xv, yv, own))
+
+        self._cb = REDUCE_CB(_cb)
+        self.staged = bool(staged_ainv)
+
+    def __enter__(self):
+        lib().orc_set_reduce_hook(self._cb, None)
+        lib().orc_set_staged_ainv(int(self.staged))
+        return self
+
+    def __exit__(self, *exc):
+        lib().orc_set_reduce_hook(REDUCE_CB(), None)
+        lib().orc_set_staged_ainv(0)
 
 
 class Matrix:

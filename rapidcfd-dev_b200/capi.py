@@ -54,7 +54,8 @@ EXPORTS = [
     "b200ldu_comm_unique_id", "b200ldu_comm_init", "b200ldu_comm_info", "b200ldu_ctx_set_stream", "b200ldu_ctx_sync",
     "b200ldu_addr_create", "b200ldu_addr_destroy", "b200ldu_addr_info", "b200ldu_addr_face_info",
     "b200ldu_addr_face_templates", "b200ldu_addr_perm",
-    "b200ldu_matrix_create", "b200ldu_matrix_set", "b200ldu_matrix_destroy",
+    "b200ldu_matrix_create", "b200ldu_matrix_set", "b200ldu_matrix_destroy", "b200ldu_matrix_debug_trace",
+    "b200ldu_matrix_debug_get",
     "b200ldu_amul", "b200ldu_tmul", "b200ldu_sumA", "b200ldu_residual", "b200ldu_H", "b200ldu_H1",
     "b200ldu_faceH", "b200ldu_precondition", "b200ldu_smooth",
     "b200ldu_vec_len", "b200ldu_to_banded", "b200ldu_from_banded", "b200ldu_amul_banded",
@@ -130,6 +131,9 @@ def lib():
     L.b200ldu_gamg_nlevels.argtypes = [vp]
     L.b200ldu_gamg_level_size.argtypes = [vp, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]
     L.b200ldu_gamg_restrict_addr.argtypes = [vp, C.c_int, vp]
+    L.b200ldu_matrix_debug_trace.argtypes = [vp, C.c_int]
+    L.b200ldu_matrix_debug_get.restype = C.c_longlong
+    L.b200ldu_matrix_debug_get.argtypes = [vp, C.c_int, vp, C.c_longlong]
     L.b200ldu_gamg_debug_get.restype = C.c_longlong
     L.b200ldu_gamg_debug_get.argtypes = [vp, C.c_int, C.c_int, vp, C.c_longlong]
     L.b200ldu_gamg_debug_invert.argtypes = [C.c_int, vp, vp]
@@ -373,6 +377,33 @@ class LduMatrix:
                                   gamg.h if gamg is not None else None, _dp(psi), _dp(source),
                                   C.byref(perf), _hp(hist) if histCap else None, histCap))
         return perf, hist[~np.isnan(hist)] if histCap else hist[:0]
+
+    # b200ldu_matrix_debug_get's codes, and the step kinds of a trace record (B200LDU_STEP_*), in order
+    TRACE_WHAT = ("records", "partials", "scalars")
+    STEP_KINDS = ("other", "init", "norm", "beta", "alpha", "end", "pcgA", "pcgB", "pcgClose", "rho", "rA0AyA",
+                  "sMag", "omega")
+    SCALARS = ("wArA", "wApA", "alpha", "beta", "omega", "rA0rA", "tAtA", "tAsA", "normFactor", "bodies", "psiBodies",
+               "steps")
+
+    def debug_trace(self, cap):
+        """Record the global sums of this handle's later solves, up to cap scalar steps per solve (0: stop)."""
+        check(lib().b200ldu_matrix_debug_trace(self.h, int(cap)))
+
+    def debug_get(self, name):
+        """HOST copy of the last solve's trace (b200ldu_matrix_debug_get): "records" float64[nRec, 16],
+        "partials" float64[nRec, P], or "scalars" as a dict of the final SolverScalars fields"""
+        what = self.TRACE_WHAT.index(name)
+        n = lib().b200ldu_matrix_debug_get(self.h, what, None, 0)
+        check(int(min(0, n)))
+        out = np.zeros(max(n, 1))
+        check(int(min(0, lib().b200ldu_matrix_debug_get(self.h, what, _hp(out), n))))
+        out = out[:n]
+        if name == "scalars":
+            return dict(zip(self.SCALARS, out.tolist()))
+        if name == "records":
+            return out.reshape(-1, 16)
+        nRec = len(self.debug_get("records"))
+        return out.reshape(nRec, -1) if nRec else out.reshape(0, 0)
 
     def solve_host(self, solver, pre, psi_h, source_h, gamg=None, **ctl):
         """End-to-end entry: HOST numpy psi/source, H2D + solve + D2H inside the call."""

@@ -1123,9 +1123,9 @@ static int gamg_cycle(Solve &S, b200ldu_gamg *g, int scaleCorrection, double *co
     TRY(scalar_step<1>(S, np, [=] __device__(SolverScalars *s) {
         s->finalResidual = s->sum[0] / s->normFactor;
         hist_put(s, hist, s->nIterations + 1, s->finalResidual);
-        bool conv = check_convergence(s);
-        s->nIterations++; // (++nIterations < maxIter && !conv) || nIterations < minIter  (:166-175)
-        bool cont = (s->nIterations < s->maxIter && !conv) || s->nIterations < s->minIter;
+        // (++nIterations < maxIter && !converged) || nIterations < minIter, short-circuited (:166-175)
+        s->nIterations++;
+        bool cont = (s->nIterations < s->maxIter && !check_convergence(s)) || s->nIterations < s->minIter;
         if (!cont) s->stop = 1;
     }));
     return B200LDU_OK;

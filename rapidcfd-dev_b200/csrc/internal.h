@@ -330,6 +330,16 @@ enum MatSlot {
     MAT_HIST,                        // device residual history
     MAT_OWN_DIAG, MAT_OWN_UPPER, MAT_OWN_LOWER, MAT_OWN_BOU, MAT_OWN_INT, // caller-order copies (matrix_set)
     MAT_VAL, MAT_VALT, MAT_FVAL,     // coefficient streams (matrix_set)
+    MAT_TRACE,                       // scalar-step trace (b200ldu_matrix_debug_trace)
+};
+
+// Where a scalar step records its sums and partials when the matrix' trace is armed (buf null: not armed).  The
+// record index is SolverScalars::traceN.  Layout: cap records of TRACE_REC doubles, then cap blocks of pstride.
+constexpr int TRACE_REC = 16;
+struct StepTrace {
+    double *buf = nullptr;
+    int cap = 0, pstride = 0;
+    int kind = B200LDU_STEP_OTHER;
 };
 
 struct b200ldu_matrix {
@@ -352,6 +362,8 @@ struct b200ldu_matrix {
                  *int_ext = nullptr;
     double *d_partials = nullptr; // reduction partials
     void *d_scal = nullptr;       // SolverScalars
+    int traceCap = 0;             // records of the armed scalar-step trace, 0: not armed
+    double *d_trace = nullptr;    // its buffer (slot MAT_TRACE)
     double *d_sendBuf = nullptr;  // packed psi at coupled-patch face cells
 };
 

@@ -17,6 +17,7 @@ struct SolverScalars {
     int maxIter, minIter, histCap, nSweeps;
     int bodies; // fused PCG: iteration bodies whose A.p product has been formed
     int psiBodies; // fused PCG: bodies whose alpha p has been added to psi (bodies - 1 or bodies)
+    int traceN;    // scalar steps with sums run so far in this solve: the next record of an armed trace (StepTrace)
     // fused PCG, deferred scalar steps (DeferredStep): steps completed (low 32 bits) | stop (bit 63), published by CTA 0 of
     // each sweep with one release store and read by every other CTA with one acquire load.  On its own 128-byte line so
     // that the waiting CTAs' polling does not slow down CTA 0's writes to the scalars above.
@@ -246,11 +247,33 @@ int ew_launch(b200ldu_ctx *ctx, int n2, const int *stop, double *partials, int *
 //    sequence number has arrived in its own mailbox and adds the contributions in rank
 //    order -- one kernel, no NCCL call, bit-identical result on every rank; or
 //  * through ncclAllReduce between a sum-only and a logic-only launch (scalar_step_on).
+// An armed trace (StepTrace): the threads of a scalar step store the partials they sum (thread t: t, t+256, ...)
+// into record sc->traceN, read before the step's barriers; thread 0 then stores the sums the logic sees and advances
+// the index.  Out of line, so that an unarmed step pays one null test and no register.
+static __device__ __noinline__ void trace_partials(const StepTrace tr, const SolverScalars *sc,
+                                                   const double *partials, int nPartials, int nred)
+{
+    const int rec = sc->traceN;
+    if (rec >= tr.cap || nPartials * nred > tr.pstride) return;
+    double *dst = tr.buf + (size_t)tr.cap * TRACE_REC + (size_t)rec * tr.pstride;
+    for (int i = threadIdx.x; i < nPartials; i += 256)
+        for (int k = 0; k < nred; k++) dst[(size_t)i * nred + k] = __ldcg(partials + (size_t)i * nred + k);
+}
+static __device__ __noinline__ void trace_record(const StepTrace tr, SolverScalars *sc, int nPartials, int nred)
+{
+    const int rec = sc->traceN++;
+    if (rec >= tr.cap) return;
+    double *r = tr.buf + (size_t)rec * TRACE_REC;
+    r[0] = tr.kind, r[1] = nred, r[2] = nPartials, r[3] = sc->nIterations;
+    for (int k = 0; k < 8; k++) r[4 + k] = k < nred ? sc->sum[k] : 0.0;
+}
+
 template <int NRED, bool RUN_LOGIC, class G>
 __device__ __forceinline__ void scalar_body(const double *partials, int nPartials, SolverScalars *sc,
-                                            G &g, const P2PRed &p2p)
+                                            G &g, const P2PRed &p2p, const StepTrace &tr)
 {
     if (NRED > 0) {
+        if (tr.buf) trace_partials(tr, sc, partials, nPartials, NRED);
         // thread t adds partials t, t+256, ... in that order (fixed => deterministic); the loads of eight of them are
         // issued together, all NRED sums of a partial at once: the step is serial time for the whole GPU
         double red[NRED > 0 ? NRED : 1];
@@ -303,16 +326,17 @@ __device__ __forceinline__ void scalar_body(const double *partials, int nPartial
         } else if (threadIdx.x == 0) {
             for (int k = 0; k < NRED; k++) sc->sum[k] = tot[k];
         }
+        if (tr.buf && threadIdx.x == 0) trace_record(tr, sc, nPartials, NRED);
     }
     if (RUN_LOGIC && threadIdx.x == 0) g(sc);
 }
 
 template <int NRED, bool RUN_LOGIC, class G>
 __global__ void __launch_bounds__(256) scalar_kernel(const double *partials, int nPartials,
-                                                     SolverScalars *sc, G g, P2PRed p2p)
+                                                     SolverScalars *sc, G g, P2PRed p2p, StepTrace tr)
 {
     if (sc->stop) return;
-    scalar_body<NRED, RUN_LOGIC>(partials, nPartials, sc, g, p2p);
+    scalar_body<NRED, RUN_LOGIC>(partials, nPartials, sc, g, p2p, tr);
 }
 
 // ---------------------------------------------------------------------------
@@ -332,6 +356,7 @@ struct DeferredStep {
     P2PRed p2p;
     unsigned want, mod; // wait until stepGen % mod == want
     int active;         // 0: nothing to close (first sweep of a solve)
+    StepTrace tr;       // the matrix' trace, when armed
     __device__ __forceinline__ bool run() const
     {
         if (!active) return *reinterpret_cast<volatile const int *>(&sc->stop) == 0;
@@ -346,7 +371,7 @@ struct DeferredStep {
                 return false;
             }
             G gg = g;
-            scalar_body<NRED, true>(partials, nPartials, sc, gg, p2p);
+            scalar_body<NRED, true>(partials, nPartials, sc, gg, p2p, tr);
             __syncthreads();
             if (threadIdx.x == 0) {
                 const unsigned long long next = ((sc->gate & 0xffffffffull) + 1) | ((unsigned long long)(sc->stop != 0) << 63);

@@ -14,18 +14,19 @@ static constexpr double VSMALL_ = 1e-300;
 P2PRed comm_p2p_red(b200ldu_ctx *ctx); // comm.cu
 
 template <int NRED, class G>
-int scalar_step_on(Solve &S, double *partials, int nPartials, G g)
+int scalar_step_on(Solve &S, double *partials, int nPartials, G g, int kind = B200LDU_STEP_OTHER)
 {
     b200ldu_ctx *ctx = S.ctx;
+    const StepTrace tr = S.trace_for(kind);
     if (ctx->nRanks == 1 || NRED == 0 || ctx->p2p) {
         P2PRed p = (ctx->nRanks > 1 && NRED > 0) ? comm_p2p_red(ctx) : P2PRed();
-        scalar_kernel<NRED, true, G><<<1, 256, 0, ctx->stream>>>(partials, nPartials, S.sc, g, p);
+        scalar_kernel<NRED, true, G><<<1, 256, 0, ctx->stream>>>(partials, nPartials, S.sc, g, p, tr);
         ctx->launches++;
     } else {
-        scalar_kernel<NRED, false, G><<<1, 256, 0, ctx->stream>>>(partials, nPartials, S.sc, g, P2PRed());
+        scalar_kernel<NRED, false, G><<<1, 256, 0, ctx->stream>>>(partials, nPartials, S.sc, g, P2PRed(), tr);
         ctx->launches++;
         TRY(comm_allreduce_sum(ctx, S.sc->sum, NRED)); // device pointer arithmetic only
-        scalar_kernel<0, true, G><<<1, 256, 0, ctx->stream>>>(partials, 0, S.sc, g, P2PRed());
+        scalar_kernel<0, true, G><<<1, 256, 0, ctx->stream>>>(partials, 0, S.sc, g, P2PRed(), StepTrace());
         ctx->launches++;
     }
     KERNEL_CHECK();
@@ -47,7 +48,9 @@ __device__ __forceinline__ void hist_put(SolverScalars *sc, double *hist, int i,
 }
 
 // ---- scalar steps shared by the Krylov solvers ----
-// end of an iteration body whose sum|r| is sum[K]: (nIterations++ < maxIter && !converged) || nIterations < minIter
+// end of an iteration body whose sum|r| is sum[K]: (nIterations++ < maxIter && !converged) || nIterations < minIter,
+// short-circuited as the reference's loop condition is: the body that reaches maxIter does not test (nor report)
+// convergence (PCG.C:190-205)
 template <int K>
 struct EndOfBody {
     double *hist;
@@ -55,10 +58,9 @@ struct EndOfBody {
     {
         sc->finalResidual = sc->sum[K] / sc->normFactor;
         hist_put(sc, hist, sc->nIterations + 1, sc->finalResidual);
-        bool conv = check_convergence(sc);
         int n = sc->nIterations;
         sc->nIterations = n + 1;
-        bool cont = (n < sc->maxIter && !conv) || (n + 1 < sc->minIter);
+        bool cont = (n < sc->maxIter && !check_convergence(sc)) || (n + 1 < sc->minIter);
         if (!cont) sc->stop = 1;
     }
 };
@@ -93,9 +95,9 @@ inline long long max_bodies(const b200ldu_controls &c) { return std::max((long l
 #define CV2(p) reinterpret_cast<const double2 *>(p)
 
 template <int NRED, class G>
-int scalar_step(Solve &S, int nPartials, G g)
+int scalar_step(Solve &S, int nPartials, G g, int kind = B200LDU_STEP_OTHER)
 {
-    return scalar_step_on<NRED>(S, S.partials, nPartials, g);
+    return scalar_step_on<NRED>(S, S.partials, nPartials, g, kind);
 }
 
 // ---------------------------------------------------------------------------

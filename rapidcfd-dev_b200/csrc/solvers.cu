@@ -37,7 +37,7 @@ int init_residual(Solve &S, const double *psi, const double *b, const double *wA
     TRY(scalar_step<2>(S, np, [=] __device__(SolverScalars *s) {
         s->sumMag0 = s->sum[0];
         s->average = s->sum[1] / s->nCellsGlobal; // gAverage: gpuFieldCommonFunctions.C:611-635
-    }));
+    }, B200LDU_STEP_INIT));
     TRY(mat_sumA(S.m, tmp, nullptr));
     const int nCells = S.m->a->nCells;
     TRY(ew_launch<1>(S.ctx, S.n2, nullptr, S.partials, &np, [=] __device__(int i, double *red) {
@@ -54,7 +54,7 @@ int init_residual(Solve &S, const double *psi, const double *b, const double *wA
         hist_put(s, hist, 0, s->finalResidual);
         bool conv = check_convergence(s);
         if (!(s->minIter > 0 || !conv)) s->stop = 1;
-    }));
+    }, B200LDU_STEP_NORM));
     return B200LDU_OK;
 }
 
@@ -77,7 +77,7 @@ int solve_pcg(Solve &S, int pk)
         int np = 0;
         // wA = M^-1 rA ; wArA = <wA, rA>
         TRY(mat_precondition(m, pk, false, rA, wA, true, nullptr, S.partials, &np, S.stop));
-        TRY(scalar_step<1>(S, np, BetaStep()));
+        TRY(scalar_step<1>(S, np, BetaStep(), B200LDU_STEP_BETA));
         // pA = wA (first) | wA + beta*pA
         TRY(ew_launch<0>(S.ctx, S.n2, S.stop, nullptr, nullptr, [=] __device__(int i, double *) {
             double2 w = CV2(wA)[i];
@@ -91,7 +91,7 @@ int solve_pcg(Solve &S, int pk)
         }));
         // wA = A pA ; wApA = <wA, pA>
         TRY(mat_amul(m, false, pA, wA, AMUL_OUT_X, nullptr, S.partials, S.stop));
-        TRY(scalar_step<1>(S, S.nBands, AlphaStep()));
+        TRY(scalar_step<1>(S, S.nBands, AlphaStep(), B200LDU_STEP_ALPHA));
         // psi += alpha pA ; rA -= alpha wA ; sum|rA|
         TRY(ew_launch<1>(S.ctx, S.n2, S.stop, S.partials, &np, [=] __device__(int i, double *red) {
             double alpha = sc->alpha;
@@ -104,7 +104,7 @@ int solve_pcg(Solve &S, int pk)
             V2(rA)[i] = r;
             red[0] += fabs(r.x) + fabs(r.y);
         }));
-        return scalar_step<1>(S, np, EndOfBody<0>{S.hist});
+        return scalar_step<1>(S, np, EndOfBody<0>{S.hist}, B200LDU_STEP_END);
     };
     return run_iterations(S, max_bodies(S.c), body);
 }
@@ -190,7 +190,8 @@ int solve_pcg_fused(Solve &S, int pk)
         }, preA);
     };
     auto preAFor = [&](long long k) {
-        return PreA{partB, nBands, sc, gB, pr, (unsigned)(2 * (k % every)), mod, k > 0 ? 1 : 0};
+        return PreA{partB, nBands, sc, gB, pr, (unsigned)(2 * (k % every)), mod, k > 0 ? 1 : 0,
+                    S.trace_for(B200LDU_STEP_PCG_B)};
     };
 
     auto body = [&](long long k) -> int {
@@ -211,7 +212,8 @@ int solve_pcg_fused(Solve &S, int pk)
         }
         int wait = 0;
         TRY(mat_halo(m, pNew, stop, &wait)); // peer-memory path: nothing is launched, the send is fused
-        const PreB preB{partA, npA, sc, gA, pr, (unsigned)(2 * (k % every) + 1), mod, 1};
+        const PreB preB{partA, npA, sc, gA, pr, (unsigned)(2 * (k % every) + 1), mod, 1,
+                        S.trace_for(B200LDU_STEP_PCG_A)};
         PcgAmulOp<PreB> op{}; // zeroes the x and aux it inherits from AmulOp and does not read
         op.stop = stop;
         op.partials = partB;
@@ -238,7 +240,7 @@ int solve_pcg_fused(Solve &S, int pk)
         } else {
             TRY(sweepAew(mb, preAFor(mb), &npA));
         }
-        TRY(scalar_step_on<2>(S, partA, npA, EndOfBody<1>{S.hist}));
+        TRY(scalar_step_on<2>(S, partA, npA, EndOfBody<1>{S.hist}, B200LDU_STEP_PCG_CLOSE));
     }
     // The last alpha p that no sweep B added to psi (the solve stopped at a judgement, converged or not): exactly
     // one update, also after a stop, so the stop flag does not gate it.  p of body j lives in pb[(j + 1) & 1], and the
@@ -273,7 +275,7 @@ int solve_pbicg(Solve &S, int pk)
         int np = 0;
         TRY(mat_precondition(m, pk, true, rT, wT, false, nullptr, nullptr, nullptr, S.stop));
         TRY(mat_precondition(m, pk, false, rA, wA, true, rT, S.partials, &np, S.stop)); // wArT = <wA, rT>
-        TRY(scalar_step<1>(S, np, BetaStep()));
+        TRY(scalar_step<1>(S, np, BetaStep(), B200LDU_STEP_BETA));
         TRY(ew_launch<0>(S.ctx, S.n2, S.stop, nullptr, nullptr, [=] __device__(int i, double *) {
             double2 w = CV2(wA)[i], wt = CV2(wT)[i];
             if (sc->nIterations == 0) {
@@ -288,7 +290,7 @@ int solve_pbicg(Solve &S, int pk)
         }));
         TRY(mat_amul(m, true, pT, wT, AMUL_ONLY, nullptr, nullptr, S.stop));
         TRY(mat_amul(m, false, pA, wA, AMUL_OUT_AUX, pT, S.partials, S.stop)); // wApT = <wA, pT>
-        TRY(scalar_step<1>(S, S.nBands, AlphaStep()));
+        TRY(scalar_step<1>(S, S.nBands, AlphaStep(), B200LDU_STEP_ALPHA));
         TRY(ew_launch<1>(S.ctx, S.n2, S.stop, S.partials, &np, [=] __device__(int i, double *red) {
             double alpha = sc->alpha;
             double2 x = CV2(psi)[i], p = CV2(pA)[i], r = CV2(rA)[i], w = CV2(wA)[i];
@@ -304,7 +306,7 @@ int solve_pbicg(Solve &S, int pk)
             V2(rT)[i] = rt;
             red[0] += fabs(r.x) + fabs(r.y);
         }));
-        return scalar_step<1>(S, np, EndOfBody<0>{S.hist});
+        return scalar_step<1>(S, np, EndOfBody<0>{S.hist}, B200LDU_STEP_END);
     };
     return run_iterations(S, max_bodies(S.c), body);
 }
@@ -351,7 +353,7 @@ int solve_pbicgstab(Solve &S, int pk)
                 }
                 s->beta = (s->rA0rA / s->rA0rAold) * (s->alpha / s->omega);
             }
-        }));
+        }, B200LDU_STEP_RHO));
         // pA = rA (first) | rA + beta*(pA - omega*AyA)
         TRY(ew_launch<0>(S.ctx, S.n2, S.stop, nullptr, nullptr, [=] __device__(int i, double *) {
             double2 r = CV2(rA)[i];
@@ -366,7 +368,8 @@ int solve_pbicgstab(Solve &S, int pk)
         }));
         TRY(mat_precondition(m, pk, false, pA, yA, false, nullptr, nullptr, nullptr, S.stop));
         TRY(mat_amul(m, false, yA, AyA, AMUL_OUT_AUX, rA0, S.partials, S.stop)); // rA0AyA
-        TRY(scalar_step<1>(S, S.nBands, [=] __device__(SolverScalars *s) { s->alpha = s->rA0rA / s->sum[0]; }));
+        TRY(scalar_step<1>(S, S.nBands, [=] __device__(SolverScalars *s) { s->alpha = s->rA0rA / s->sum[0]; },
+                           B200LDU_STEP_RA0AYA));
         // sA = rA - alpha*AyA ; psi += alpha*yA (both exits of the body need it) ; sum|sA|
         TRY(ew_launch<1>(S.ctx, S.n2, S.stop, S.partials, &np, [=] __device__(int i, double *red) {
             double alpha = sc->alpha;
@@ -383,10 +386,14 @@ int solve_pbicgstab(Solve &S, int pk)
                 hist_put(s, hist, s->nIterations, s->finalResidual);
                 s->stop = 1;
             }
-        }));
+        }, B200LDU_STEP_SMAG));
         TRY(mat_precondition(m, pk, false, sA, zA, false, nullptr, nullptr, nullptr, S.stop));
         TRY(mat_amul(m, false, zA, tA, AMUL_OUT_OUT_OUT_AUX, sA, S.partials, S.stop)); // tAtA, tAsA
-        TRY(scalar_step<2>(S, S.nBands, [=] __device__(SolverScalars *s) { s->omega = s->sum[1] / s->sum[0]; }));
+        TRY(scalar_step<2>(S, S.nBands, [=] __device__(SolverScalars *s) {
+            s->tAtA = s->sum[0];
+            s->tAsA = s->sum[1];
+            s->omega = s->tAsA / s->tAtA;
+        }, B200LDU_STEP_OMEGA));
         TRY(ew_launch<1>(S.ctx, S.n2, S.stop, S.partials, &np, [=] __device__(int i, double *red) {
             double omega = sc->omega;
             const double *second = quirk ? yA : zA; // PBiCGStab.C:263-270 passes yA
@@ -396,7 +403,7 @@ int solve_pbicgstab(Solve &S, int pk)
             V2(rA)[i] = r;
             red[0] += fabs(r.x) + fabs(r.y);
         }));
-        return scalar_step<1>(S, np, EndOfBody<0>{hist});
+        return scalar_step<1>(S, np, EndOfBody<0>{hist}, B200LDU_STEP_END);
     };
     return run_iterations(S, max_bodies(S.c), body);
 }
@@ -434,11 +441,12 @@ int solve_smooth(Solve &S)
             s->finalResidual = s->sum[0] / s->normFactor;
             int k = s->nIterations / (nSweeps > 0 ? nSweeps : 1) + 1;
             hist_put(s, hist, k, s->finalResidual);
-            bool conv = check_convergence(s);
-            s->nIterations += nSweeps; // ((nIterations += nSweeps) < maxIter && !conv) || nIterations < minIter
-            bool cont = (s->nIterations < s->maxIter && !conv) || s->nIterations < s->minIter;
+            // ((nIterations += nSweeps) < maxIter && !converged) || nIterations < minIter, short-circuited
+            // (smoothSolver.C:182-187)
+            s->nIterations += nSweeps;
+            bool cont = (s->nIterations < s->maxIter && !check_convergence(s)) || s->nIterations < s->minIter;
             if (!cont) s->stop = 1;
-        });
+        }, B200LDU_STEP_END);
     };
     int per = nSweeps > 0 ? nSweeps : 1;
     long long maxBodies = ((long long)(S.c.maxIter > S.c.minIter ? S.c.maxIter : S.c.minIter) + per - 1) / per + 1;
@@ -474,9 +482,17 @@ Solve::Solve(b200ldu_matrix *mat, const b200ldu_controls &controls, double *psi_
     rc = open(nIterations0, converged0);
 }
 
+// doubles of partials a trace record keeps: what the largest scalar step sums (the fused PCG's two partial buffers)
+static int trace_pstride(const b200ldu_matrix *m)
+{
+    const b200ldu_addr *a = m->a;
+    return 2 * std::max(a->L.nBands, a->ctx->smCount * 8);
+}
+
 int Solve::open(int nIterations0, int converged0)
 {
     if (histCap > 0) TRY(m->mem.slot(MAT_HIST, hist, (size_t)histCap));
+    if (m->traceCap > 0) trace = StepTrace{m->d_trace, m->traceCap, trace_pstride(m), B200LDU_STEP_OTHER};
     entered_ = true;
     if (++solveDepth > SOLVE_MAX_DEPTH) {
         b200_set_error("solve: nesting too deep");
@@ -667,6 +683,43 @@ int solve_banded(b200ldu_matrix *m, const char *solver, const char *pre, const b
         return rc;
     }
     return S.finish(perf, hist_h, resultBuf);
+}
+
+extern "C" int b200ldu_matrix_debug_trace(b200ldu_matrix *m, int cap)
+{
+    if (!m || cap < 0) return B200LDU_EINVAL;
+    CUDA_TRY(cudaSetDevice(m->a->ctx->device));
+    if (cap > 0) TRY(m->mem.slot(MAT_TRACE, m->d_trace, (size_t)cap * (TRACE_REC + trace_pstride(m))));
+    m->traceCap = cap;
+    return B200LDU_OK;
+}
+
+// Read-only: waits for the context's stream and copies; the trace of a later solve starts again at record 0.
+extern "C" long long b200ldu_matrix_debug_get(const b200ldu_matrix *m, int what, double *out_h, long long cap)
+{
+    if (!m || what < B200LDU_TRACE_RECORDS || what > B200LDU_TRACE_SCALARS) return B200LDU_EINVAL;
+    b200ldu_ctx *ctx = m->a->ctx;
+    if (cudaSetDevice(ctx->device) != cudaSuccess || cudaStreamSynchronize(ctx->stream) != cudaSuccess)
+        return B200LDU_ECUDA;
+    SolverScalars h;
+    if (cudaMemcpy(&h, m->d_scal, sizeof(h), cudaMemcpyDeviceToHost) != cudaSuccess) return B200LDU_ECUDA;
+    cap = std::max(cap, 0LL);
+    if (what == B200LDU_TRACE_SCALARS) {
+        const double v[12] = {h.wArA, h.wApA, h.alpha, h.beta, h.omega, h.rA0rA, h.tAtA, h.tAsA, h.normFactor,
+                              (double)h.bodies, (double)h.psiBodies, (double)h.traceN};
+        if (out_h) memcpy(out_h, v, sizeof(double) * (size_t)std::min(cap, 12LL));
+        return 12;
+    }
+    const double *buf = m->d_trace;
+    const long long nRec = std::min(h.traceN, m->traceCap);
+    if (m->traceCap == 0) return 0;
+    const long long per = what == B200LDU_TRACE_RECORDS ? TRACE_REC : trace_pstride(m);
+    const long long n = nRec * per;
+    const double *src = buf + (what == B200LDU_TRACE_RECORDS ? 0 : (size_t)m->traceCap * TRACE_REC);
+    if (out_h && n > 0 &&
+        cudaMemcpy(out_h, src, sizeof(double) * (size_t)std::min(n, cap), cudaMemcpyDeviceToHost) != cudaSuccess)
+        return B200LDU_ECUDA;
+    return n;
 }
 
 extern "C" int b200ldu_solve(b200ldu_matrix *m, const char *solver, const char *pre,

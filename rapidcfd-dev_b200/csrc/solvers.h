@@ -42,6 +42,13 @@ struct Solve {
     cudaEvent_t ev[2] = {nullptr, nullptr};
     bool useGraph = false; // replay iteration chunks as a CUDA graph
     SolveResult result;
+    StepTrace trace;        // the matrix' scalar-step trace (buf null: not armed)
+    StepTrace trace_for(int kind) const
+    {
+        StepTrace t = trace;
+        t.kind = kind;
+        return t;
+    }
 
   private:
     int open(int nIterations0, int converged0);
